@@ -14,10 +14,6 @@ FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c
          "--threads", "4"]
 
 
-if os.environ.get("HV_BUILD_TUNING", "0") == "1":   # A/B switches through HV_* environment variables (csrc/tuning.h); never in the release library
-    FLAGS.append("-DHV_TUNING")
-
-
 def sources():
     return sorted(os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cu", ".cpp")))
 

@@ -13,7 +13,6 @@
 #include <stdlib.h>
 
 #include "ptx.cuh"
-#include "tuning.h"
 #include "tma.h"
 
 namespace hv {
@@ -421,10 +420,9 @@ cudaError_t launch_temporal_attention(const __half* qkv, __half* out, int B, int
   const int wpb = 8;
   const unsigned grid = static_cast<unsigned>((nprob + wpb - 1) / wpb);
   const float scale_log2 = 1.4426950408889634f / sqrtf(static_cast<float>(d));
-  static const int use_tma = static_cast<int>(tune_env("HV_TATTN_TMA", 1));
   // the two high-resolution levels; small problems keep the register kernel.  The choice depends on HW only, not on the batch size
   // (a one-half unit of the multi-GPU split must run the same kernel as that half of a CFG batch).
-  if (use_tma && static_cast<long long>(HW) * heads >= 2048) {
+  if (static_cast<long long>(HW) * heads >= 2048) {
     if (d == 40 && heads % 2 == 0) return launch_tt<40, 2>(qkv, out, B, F, HW, heads, scale_log2, stream);
     if (d == 80) return launch_tt<80, 1>(qkv, out, B, F, HW, heads, scale_log2, stream);
   }

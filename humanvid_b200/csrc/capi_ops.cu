@@ -64,13 +64,13 @@ int hv_op_conv3x3_direct(const void* X, const void* W, const void* bias, void* o
 }
 
 size_t hv_groupnorm_scratch_floats(int64_t C, int64_t NF, int64_t HW, int32_t groups) {
-  return groupnorm_scratch_floats((int)C, (int)NF, (int)HW, groups, device_sms() ? device_sms() : 132);
+  return groupnorm_scratch_floats((int)C, (int)NF, (int)HW, groups);
 }
 
 int hv_op_groupnorm(const void* X, int64_t C1, const void* X2, int64_t C2, const void* gamma, const void* beta, void* out,
                     int64_t NF, int64_t HW, int32_t groups, float eps, int32_t silu, float* stats, hv_stream_t stream) {
   if (!device_sms()) return HV_ERR_CUDA;
-  CK(launch_groupnorm(H(X), (int)C1, H(X2), (int)C2, H(gamma), H(beta), HM(out), (int)NF, (int)HW, groups, eps, silu, stats, device_sms(), ST(stream)),
+  CK(launch_groupnorm(H(X), (int)C1, H(X2), (int)C2, H(gamma), H(beta), HM(out), (int)NF, (int)HW, groups, eps, silu, stats, ST(stream)),
      "hv_op_groupnorm");
 }
 
@@ -107,14 +107,6 @@ int hv_op_ncfhw_to_nhwc(const void* X, void* out, int64_t B, int64_t C, int64_t 
 }
 int hv_op_nhwc_to_ncfhw(const void* X, int64_t ldx, void* out, int64_t B, int64_t C, int64_t F, int64_t Hh, int64_t W, hv_stream_t stream) {
   CK(launch_nhwc_to_ncfhw(H(X), (int)ldx, HM(out), (int)B, (int)C, (int)F, (int)Hh, (int)W, ST(stream)), "hv_op_nhwc_to_ncfhw");
-}
-int hv_op_upsample2x(const void* X, void* out, int64_t NF, int64_t Hh, int64_t W, int64_t C, hv_stream_t stream) {
-  if (!device_sms()) return HV_ERR_CUDA;
-  CK(launch_upsample2x(H(X), HM(out), NF, (int)Hh, (int)W, (int)C, device_sms(), ST(stream)), "hv_op_upsample2x");
-}
-int hv_op_add(const void* A, const void* B, void* out, int64_t n, hv_stream_t stream) {
-  if (!device_sms()) return HV_ERR_CUDA;
-  CK(launch_add(H(A), H(B), HM(out), n, device_sms(), ST(stream)), "hv_op_add");
 }
 int hv_op_pixel_unshuffle(const void* X, void* out, int64_t B, int64_t C, int64_t F, int64_t Hh, int64_t W, int32_t r, hv_stream_t stream) {
   if (!device_sms()) return HV_ERR_CUDA;

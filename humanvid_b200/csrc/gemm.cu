@@ -18,7 +18,6 @@
 
 #include "gemm.cuh"
 #include "ptx.cuh"
-#include "tuning.h"
 #include "wgmma.cuh"
 
 namespace hv {
@@ -352,8 +351,7 @@ cudaError_t launch_gemm(const CUtensorMap& a0, const CUtensorMap& a1, const CUte
   if (p.b_batch && (e.bias || e.rowvec || e.residual || e.geglu || (p.b_out_stride % 8))) return cudaErrorInvalidValue;
   if (e.geglu && block_n != 256) return cudaErrorInvalidValue;
   const int grid = tiles < num_sms ? tiles : num_sms;
-  static const int bst_env = static_cast<int>(tune_env("HV_GEMM_BST", 1));
-  if (bst_env && p.a_mode == A_LINEAR && !p.b_batch && n_tiles <= num_sms) {
+  if (p.a_mode == A_LINEAR && !p.b_batch && n_tiles <= num_sms) {
     cudaError_t r = cudaErrorNotSupported;
     if (block_n == 256) r = launch_bst<256>(a0, a1, b, p, e, m_tiles, n_tiles, num_sms, stream);
     if (block_n == 160) r = launch_bst<160>(a0, a1, b, p, e, m_tiles, n_tiles, num_sms, stream);

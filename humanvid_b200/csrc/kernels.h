@@ -6,10 +6,8 @@
 namespace hv {
 
 cudaError_t launch_groupnorm(const __half* x1, int C1, const __half* x2, int C2, const __half* gamma, const __half* beta,
-                             __half* out, int NF, int HW, int groups, float eps, int silu, float* stats, int num_sms,
-                             cudaStream_t stream);
-size_t groupnorm_scratch_floats(int C, int NF, int HW, int groups, int num_sms);
-int groupnorm_num_launches(int C, int NF, int HW, int num_sms);
+                             __half* out, int NF, int HW, int groups, float eps, int silu, float* stats, cudaStream_t stream);
+size_t groupnorm_scratch_floats(int C, int NF, int HW, int groups);
 cudaError_t launch_layernorm(const __half* x, const __half* gamma, const __half* beta, __half* out, long long rows, int C, float eps,
                              const __half* pre_add, long long rows_per_group, __half* x_out, const __half* pe, int hw, int F,
                              cudaStream_t stream);
@@ -28,8 +26,6 @@ cudaError_t launch_attention(const AttnArgs& a, int num_sms, cudaStream_t stream
 
 cudaError_t launch_ncfhw_to_nhwc(const void* x, __half* out, int B, int C, int F, int H, int W, int src_fp32, cudaStream_t s, int ldo = 0);
 cudaError_t launch_nhwc_to_ncfhw(const __half* x, int ldx, __half* out, int B, int C, int F, int H, int W, cudaStream_t s);
-cudaError_t launch_upsample2x(const __half* x, __half* out, long long NF, int H, int W, int C, int num_sms, cudaStream_t s);
-cudaError_t launch_add(const __half* a, const __half* b, __half* out, long long n, int num_sms, cudaStream_t s);
 cudaError_t launch_pixel_unshuffle(const __half* x, __half* out, int B, int C, int F, int H, int W, int r, int num_sms, cudaStream_t s);
 cudaError_t launch_plucker_unshuffle(const float* K, const float* c2w, __half* out, long long NF, int H, int W, int r, int num_sms, cudaStream_t s);
 cudaError_t launch_small_linear(const __half* x, const __half* w, const __half* bias, __half* out, int M, int N, int K, int act_in,

@@ -1,6 +1,6 @@
-// Glue kernels of the denoising path: layout changes at the (B,C,F,H,W) boundary, nearest upsampling, the tiny
-// linears of the time embedding / cross-attention collapse, small-channel direct convolutions (conv_in, PoseGuider),
-// weight packing, and a slow CUDA-core GEMM used only to localise faults in tests.
+// Glue kernels of the denoising path: layout changes at the (B,C,F,H,W) boundary, pixel unshuffle and the Plucker producer of
+// the camera encoder, the tiny linears of the time embedding / cross-attention collapse, the timestep embedding, small-channel
+// direct convolutions (PoseGuider conv_in), weight packing, and a slow CUDA-core GEMM used only to localise faults in tests.
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -50,27 +50,6 @@ __global__ void nhwc_to_ncfhw_kernel(const __half* __restrict__ x, int ldx, __ha
   for (int i = threadIdx.y; i < 32; i += blockDim.y) {
     const int c = c0 + i, p = p0 + threadIdx.x;
     if (c < C && p < HW) out[((static_cast<long long>(b) * C + c) * F + f) * HW + p] = tile[threadIdx.x][i];
-  }
-}
-
-__global__ void upsample2x_kernel(const uint4* __restrict__ x, uint4* __restrict__ out, long long total, int H, int W, int vecs) {
-  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
-       i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const int v = static_cast<int>(i % vecs);
-    long long r = i / vecs;
-    const int xo = static_cast<int>(r % (2 * W));
-    r /= 2 * W;
-    const int yo = static_cast<int>(r % (2 * H));
-    const long long n = r / (2 * H);
-    out[i] = __ldg(&x[((n * H + (yo >> 1)) * W + (xo >> 1)) * vecs + v]);
-  }
-}
-
-__global__ void add_kernel(const __half2* __restrict__ a, const __half2* __restrict__ b, __half2* __restrict__ out, long long n2) {
-  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n2;
-       i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    float2 fa = __half22float2(a[i]), fb = __half22float2(b[i]);
-    out[i] = __floats2half2_rn(fa.x + fb.x, fa.y + fb.y);
   }
 }
 
@@ -297,17 +276,6 @@ cudaError_t launch_nhwc_to_ncfhw(const __half* x, int ldx, __half* out, int B, i
   const int HW = H * W;
   dim3 grid((HW + 31) / 32, (C + 31) / 32, B * F), block(32, 8);
   nhwc_to_ncfhw_kernel<<<grid, block, 0, s>>>(x, ldx, out, B, C, F, HW);
-  HV_LAUNCH_CHECK();
-}
-cudaError_t launch_upsample2x(const __half* x, __half* out, long long NF, int H, int W, int C, int num_sms, cudaStream_t s) {
-  const int vecs = C / 8;
-  const long long total = NF * 4LL * H * W * vecs;
-  upsample2x_kernel<<<blocks_for(total, num_sms), kThreads, 0, s>>>(reinterpret_cast<const uint4*>(x), reinterpret_cast<uint4*>(out), total, H, W, vecs);
-  HV_LAUNCH_CHECK();
-}
-cudaError_t launch_add(const __half* a, const __half* b, __half* out, long long n, int num_sms, cudaStream_t s) {
-  add_kernel<<<blocks_for(n / 2, num_sms), kThreads, 0, s>>>(reinterpret_cast<const __half2*>(a), reinterpret_cast<const __half2*>(b),
-                                                             reinterpret_cast<__half2*>(out), n / 2);
   HV_LAUNCH_CHECK();
 }
 cudaError_t launch_pixel_unshuffle(const __half* x, __half* out, int B, int C, int F, int H, int W, int r, int num_sms, cudaStream_t s) {

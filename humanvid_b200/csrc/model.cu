@@ -179,16 +179,14 @@ struct hv_model {
   struct TapInfo { std::string name; int NF, H, W, C; };
   std::vector<TapInfo> tap_list;
   std::vector<void*> tap_dst;
-  void tap(const std::string& name, const Tens& t) {
+  void tap(const std::string& name, const Tens& t) {   // records the plan entry in the planning pass too (hv_debug_tap_count)
     const size_t i = tap_list.size();
     tap_list.push_back({name, t.NF, t.H, t.W, t.C});
-    if (!ar.dry && i < tap_dst.size() && tap_dst[i] != nullptr) {
-      launches += 1;
-      ck(cudaMemcpyAsync(tap_dst[i], t.p, static_cast<size_t>(t.numel()) * 2, cudaMemcpyDeviceToDevice, st), "tap copy");
-    }
+    if (i < tap_dst.size() && tap_dst[i] != nullptr)
+      launch(1, {}, [&] { ck(cudaMemcpyAsync(tap_dst[i], t.p, static_cast<size_t>(t.numel()) * 2, cudaMemcpyDeviceToDevice, st), "tap copy"); });
   }
-  // optional per-category device timing (bench.py's roofline): events bracket every operator launch
-  enum Cat { CAT_GEMM = 0, CAT_CONV = 1, CAT_ATTN = 2, CAT_TATTN = 3, CAT_NORM = 4, CAT_MISC = 5, CAT_N = 6 };
+  // optional per-category device timing (bench.py's roofline): events bracket every categorised operator launch
+  enum Cat { CAT_NONE = -1, CAT_GEMM = 0, CAT_CONV = 1, CAT_ATTN = 2, CAT_TATTN = 3, CAT_NORM = 4, CAT_MISC = 5, CAT_N = 6 };
   bool profiling = false;
   struct Rec { int cat; cudaEvent_t a, b; double flops; long long m, n, k; const char* label; };
   std::vector<Rec> recs;
@@ -202,25 +200,40 @@ struct hv_model {
     }
     return ev_pool[ev_used++];
   }
-  struct Timed {  // RAII bracket around one operator
-    hv_model* m; int cat; double flops; long long M, N, K; const char* label; cudaEvent_t a{};
-    Timed(hv_model* mm, int c, double f, const char* lb = "", long long M_ = 0, long long N_ = 0, long long K_ = 0)
-        : m(mm), cat(c), flops(f), M(M_), N(N_), K(K_), label(lb) {
-      if (m->profiling && !m->ar.dry) { a = m->ev(); cudaEventRecord(a, m->st); }
+  // the profile row of one operator; CAT_NONE: counted, not timed
+  struct Op { int cat = CAT_NONE; const char* label = ""; double flops = 0; long long M = 0, N = 0, K = 0; };
+  // The one path of device work in a forward: fn issues `n` launches (kernels, memsets, copies).  The planning pass only sizes the
+  // workspace (ar.base is null), so nothing is issued in it.
+  template <class Fn> void launch(int n, const Op& op, Fn&& fn) {
+    if (ar.dry) return;
+    launches += n;
+    if (!profiling || op.cat == CAT_NONE) {
+      fn();
+      return;
     }
-    ~Timed() {
-      if (m->profiling && !m->ar.dry) { cudaEvent_t b = m->ev(); cudaEventRecord(b, m->st); m->recs.push_back({cat, a, b, flops, M, N, K, label}); }
-    }
-  };
+    cudaEvent_t a = ev();
+    cudaEventRecord(a, st);
+    fn();
+    cudaEvent_t b = ev();
+    cudaEventRecord(b, st);
+    recs.push_back({op.cat, a, b, op.flops, op.M, op.N, op.K, op.label});
+  }
 
   // ---- UNet
   Conv3 conv_in;  // 4 input channels zero-padded to 64: runs on the implicit-GEMM kernel
   Lin te1, te2;
-  struct DownBlk { std::vector<ResnetW> res; std::vector<SpatialW> attn; std::vector<MotionW> mm; bool has_down = false; Conv3 down; };
-  struct UpBlk { std::vector<ResnetW> res; std::vector<SpatialW> attn; std::vector<MotionW> mm; bool has_up = false; Conv3 up; };
-  std::vector<DownBlk> down;
-  struct { std::vector<ResnetW> res; std::vector<SpatialW> attn; std::vector<MotionW> mm; } mid;
-  std::vector<UpBlk> up;
+  // down_blocks.i / mid_block / up_blocks.i: layer j is res[j], then attn[j] and mm[j] where present, and the stage ends in an
+  // optional down- or up-sampler conv
+  struct Stage {
+    std::string name;
+    std::vector<ResnetW> res;
+    std::vector<SpatialW> attn;
+    std::vector<MotionW> mm;
+    bool has_sampler = false;
+    Conv3 sampler;
+  };
+  std::vector<Stage> down, up;
+  Stage mid;
   Norm norm_out;
   Conv3 conv_out;
   std::vector<SpatialW*> readers;  // reference-bank order
@@ -285,27 +298,33 @@ struct hv_model {
     if (bias) l.bias = vec(pfx + ".bias", out);
     return l;
   }
-  Conv3 conv3(const std::string& pfx, int cout, int cin, bool bias = true, bool pad_out_64 = false) {
+  const Raw& conv3_weight(const std::string& pfx, int cout, int cin) {
     const Raw& r = get(pfx + ".weight");
     if (r.shape.size() != 4 || r.shape[0] != cout || r.shape[1] != cin || r.shape[2] != 3 || r.shape[3] != 3)
       fail(HV_ERR_INVALID, "weight '%s.weight' is not (%d,%d,3,3)", pfx.c_str(), cout, cin);
+    return r;
+  }
+  // Channel padding of a packed [cout_pad][9 * cin_pad] 3x3 conv.  The implicit-GEMM kernel reads 64-channel k-blocks and writes
+  // cout rounded up to 8 (PAD_OUT_64: to 64, the output feeds another implicit-GEMM conv); the small-channel kernel (smallconv.cu)
+  // takes the true channel counts (PAD_NONE).
+  enum ConvPad { PAD_GEMM, PAD_OUT_64, PAD_NONE };
+  Conv3 conv3(const std::string& pfx, int cout, int cin, ConvPad pad = PAD_GEMM) {
+    const Raw& r = conv3_weight(pfx, cout, cin);
     Conv3 c;
     c.cin = cin;
     c.cout = cout;
-    c.cin_pad = static_cast<int>(rup(cin, 64));
-    c.cout_pad = static_cast<int>(pad_out_64 ? rup(cout, 64) : rup(cout, 8));  // pad_out_64: the output feeds another implicit-GEMM conv
+    c.cin_pad = pad == PAD_NONE ? cin : static_cast<int>(rup(cin, 64));
+    c.cout_pad = pad == PAD_NONE ? cout : static_cast<int>(rup(cout, pad == PAD_OUT_64 ? 64 : 8));
     c.w.rows = c.cout_pad;
     c.w.cols = 9LL * c.cin_pad;
     c.w.p = dmalloc(c.w.rows * c.w.cols);
     ck(launch_pack_conv3x3(r.p, c.w.p, cout, cin, c.cout_pad, c.cin_pad, sms, st), "pack conv3x3");
-    if (bias) c.bias = vec(pfx + ".bias", cout, c.cout_pad);
+    c.bias = vec(pfx + ".bias", cout, c.cout_pad);
     return c;
   }
   // Upsample3D's conv packed for op_upconv2x2: [4 parities][cout][4 * cin]
   Conv3 upconv(const std::string& pfx, int cout, int cin) {
-    const Raw& r = get(pfx + ".weight");
-    if (r.shape.size() != 4 || r.shape[0] != cout || r.shape[1] != cin || r.shape[2] != 3 || r.shape[3] != 3)
-      fail(HV_ERR_INVALID, "weight '%s.weight' is not (%d,%d,3,3)", pfx.c_str(), cout, cin);
+    const Raw& r = conv3_weight(pfx, cout, cin);
     if ((cin % 64) || (cout % 8)) fail(HV_ERR_INVALID, "upsampler conv '%s': %d -> %d channels must be multiples of 64 / 8", pfx.c_str(), cin, cout);
     Conv3 c;
     c.cin = c.cin_pad = cin;
@@ -387,7 +406,7 @@ struct hv_model {
     s.ff2 = lin(b + ".ff.net.2", C, 4 * C);
     return s;
   }
-  TAttnW tattn(const std::string& attn_pfx, const std::string& norm_pfx, int C, int max_len) {
+  TAttnW tattn(const std::string& attn_pfx, const std::string& norm_pfx, int C) {
     TAttnW t;
     t.ln = norm(norm_pfx, C, 1e-5f);
     t.wqkv = Mat{dmalloc(3LL * C * C), 3LL * C, C};
@@ -400,7 +419,6 @@ struct hv_model {
     if (pe.numel() % C) fail(HV_ERR_INVALID, "'%s.pos_encoder.pe' width != %d", attn_pfx.c_str(), C);
     t.pe = pe.p;
     t.max_len = static_cast<int>(pe.numel() / C);
-    (void)max_len;
     return t;
   }
   MotionW motion(const std::string& pfx, int C) {
@@ -414,11 +432,24 @@ struct hv_model {
     m.proj_out = lin(t + ".proj_out", C, C);
     const std::string b = t + ".transformer_blocks.0";
     for (int i = 0; i < 2; ++i)
-      m.attn.push_back(tattn(b + ".attention_blocks." + std::to_string(i), b + ".norms." + std::to_string(i), C, cfg.motion_max_len));
+      m.attn.push_back(tattn(b + ".attention_blocks." + std::to_string(i), b + ".norms." + std::to_string(i), C));
     m.ffn = norm(b + ".ff_norm", C, 1e-5f);
     m.ff1 = ff1_geglu(b + ".ff.net.0.proj", C);
     m.ff2 = lin(b + ".ff.net.2", C, 4 * C);
     return m;
+  }
+
+  // layer j: a resnet ins[j] -> C channels, then a transformer if j < n_attn and a motion module if j < n_mm
+  Stage stage(const std::string& name, const std::vector<int>& ins, int C, int temb, size_t n_attn, size_t n_mm) {
+    Stage s;
+    s.name = name;
+    for (size_t j = 0; j < ins.size(); ++j) {
+      const std::string sj = "." + std::to_string(j);
+      s.res.push_back(resnet(name + ".resnets" + sj, ins[j], C, temb));
+      if (j < n_attn) s.attn.push_back(spatial(name + ".attentions" + sj, C));
+      if (j < n_mm) s.mm.push_back(motion(name + ".motion_modules" + sj, C));
+    }
+    return s;
   }
 
   void build_unet() {
@@ -428,39 +459,25 @@ struct hv_model {
     conv_in = conv3("conv_in", ch[0], cfg.in_channels);
     te1 = lin("time_embedding.linear_1", temb, ch[0]);
     te2 = lin("time_embedding.linear_2", temb, temb);
+    down.clear();
+    up.clear();
     int prev = ch[0];
-    down.resize(4);
     for (int i = 0; i < 4; ++i) {
-      auto& d = down[i];
-      const std::string p = "down_blocks." + std::to_string(i);
-      for (int j = 0; j < 2; ++j) {
-        d.res.push_back(resnet(p + ".resnets." + std::to_string(j), j == 0 ? prev : ch[i], ch[i], temb));
-        if (i < 3) d.attn.push_back(spatial(p + ".attentions." + std::to_string(j), ch[i]));
-        if (mm) d.mm.push_back(motion(p + ".motion_modules." + std::to_string(j), ch[i]));
-      }
-      d.has_down = i < 3;
-      if (d.has_down) d.down = conv3(p + ".downsamplers.0.conv", ch[i], ch[i]);
+      Stage s = stage("down_blocks." + std::to_string(i), {prev, ch[i]}, ch[i], temb, i < 3 ? 2 : 0, mm ? 2 : 0);
+      s.has_sampler = i < 3;
+      if (s.has_sampler) s.sampler = conv3(s.name + ".downsamplers.0.conv", ch[i], ch[i]);
+      down.push_back(std::move(s));
       prev = ch[i];
     }
-    mid.res.push_back(resnet("mid_block.resnets.0", ch[3], ch[3], temb));
-    mid.res.push_back(resnet("mid_block.resnets.1", ch[3], ch[3], temb));
-    mid.attn.push_back(spatial("mid_block.attentions.0", ch[3]));
-    if (mm) mid.mm.push_back(motion("mid_block.motion_modules.0", ch[3]));
+    mid = stage("mid_block", {ch[3], ch[3]}, ch[3], temb, 1, mm ? 1 : 0);
     const int rev[4] = {ch[3], ch[2], ch[1], ch[0]};
-    up.resize(4);
     prev = rev[0];
     for (int i = 0; i < 4; ++i) {
-      auto& u = up[i];
-      const std::string p = "up_blocks." + std::to_string(i);
-      const int c = rev[i], cin = rev[std::min(i + 1, 3)];
-      for (int j = 0; j < 3; ++j) {
-        const int rin = (j == 0 ? prev : c) + (j == 2 ? cin : c);
-        u.res.push_back(resnet(p + ".resnets." + std::to_string(j), rin, c, temb));
-        if (i > 0) u.attn.push_back(spatial(p + ".attentions." + std::to_string(j), c));
-        if (mm) u.mm.push_back(motion(p + ".motion_modules." + std::to_string(j), c));
-      }
-      u.has_up = i < 3;
-      if (u.has_up) u.up = upconv(p + ".upsamplers.0.conv", c, c);
+      const int c = rev[i], skip = rev[std::min(i + 1, 3)];   // resnet j reads h ++ the j-th skip from the end
+      Stage s = stage("up_blocks." + std::to_string(i), {prev + c, c + c, c + skip}, c, temb, i > 0 ? 3 : 0, mm ? 3 : 0);
+      s.has_sampler = i < 3;
+      if (s.has_sampler) s.sampler = upconv(s.name + ".upsamplers.0.conv", c, c);
+      up.push_back(std::move(s));
       prev = c;
     }
     if (cfg.kind == HV_KIND_UNET3D) {   // the reference ("writer") 2-D UNet has its post-process removed (unet_2d_condition.py:1295-1299)
@@ -474,22 +491,6 @@ struct hv_model {
     for (auto& a : mid.attn) readers.push_back(&a);
     std::stable_sort(readers.begin(), readers.end(), [](const SpatialW* x, const SpatialW* y) { return x->C > y->C; });
     for (size_t i = 0; i < readers.size(); ++i) readers[i]->reader_idx = static_cast<int>(i);
-  }
-
-  // unpadded [cout][9 * cin] packing for the small-channel kernel
-  Conv3 conv3_small(const std::string& pfx, int cout, int cin) {
-    const Raw& r = get(pfx + ".weight");
-    if (r.shape.size() != 4 || r.shape[0] != cout || r.shape[1] != cin || r.shape[2] != 3 || r.shape[3] != 3)
-      fail(HV_ERR_INVALID, "weight '%s.weight' is not (%d,%d,3,3)", pfx.c_str(), cout, cin);
-    Conv3 c;
-    c.cin = c.cin_pad = cin;
-    c.cout = c.cout_pad = cout;
-    c.w.rows = cout;
-    c.w.cols = 9LL * cin;
-    c.w.p = dmalloc(c.w.rows * c.w.cols);
-    ck(launch_pack_conv3x3(r.p, c.w.p, cout, cin, cout, cin, sms, st), "pack small conv3x3");
-    c.bias = vec(pfx + ".bias", cout);
-    return c;
   }
 
   void build_pose_guider() {
@@ -508,7 +509,7 @@ struct hv_model {
         const std::string name = "blocks." + std::to_string(2 * i + k);
         chain = chain && smallconv_supported(cin, cout, stride);
         pg_small.push_back(chain);
-        pg_convs.push_back(chain ? conv3_small(name, cout, cin) : conv3(name, cout, cin, true, true));
+        pg_convs.push_back(conv3(name, cout, cin, chain ? PAD_NONE : PAD_OUT_64));
         pg_strides.push_back(stride);
       }
     }
@@ -531,7 +532,7 @@ struct hv_model {
       m.C = C;
       m.heads = cfg.cam_heads;
       m.d = C / cfg.cam_heads;
-      m.attn.push_back(tattn(a + ".attention_blocks.0", a + ".norms.0", C, cfg.cam_max_len));
+      m.attn.push_back(tattn(a + ".attention_blocks.0", a + ".norms.0", C));
       m.ffn = norm(a + ".ff_norm", C, 1e-5f);
       m.ff1 = ff1_geglu(a + ".ff.net.0.proj", C);
       m.ff2 = lin(a + ".ff.net.2", C, 4 * C);
@@ -553,31 +554,28 @@ struct hv_model {
     const int C2 = x2 ? x2->C : 0;
     if (n.C != x.C + C2) fail(HV_ERR_INVALID, "groupnorm width %d != %d + %d", n.C, x.C, C2);
     Tens out = alloc_act(x.NF, x.H, x.W, x.C + C2);
-    float* stats = static_cast<float*>(ar.alloc(sizeof(float) * groupnorm_scratch_floats(x.C + C2, x.NF, x.H * x.W, cfg.norm_groups, sms)));
-    if (ar.dry) return out;
-    launches += groupnorm_num_launches(x.C + C2, x.NF, x.H * x.W, sms);
-    Timed tm(this, CAT_NORM, 0, "groupnorm", x.rows(), x.C + C2, 0);
-    ck(launch_groupnorm(x.p, x.C, x2 ? x2->p : nullptr, C2, n.g, n.b, out.p, x.NF, x.H * x.W, cfg.norm_groups, n.eps, silu ? 1 : 0, stats, sms, st),
-       "groupnorm");
+    float* stats = static_cast<float*>(ar.alloc(sizeof(float) * groupnorm_scratch_floats(x.C + C2, x.NF, x.H * x.W, cfg.norm_groups)));
+    launch(2, {CAT_NORM, "groupnorm", 0, x.rows(), x.C + C2, 0}, [&] {   // statistics + apply
+      ck(launch_groupnorm(x.p, x.C, x2 ? x2->p : nullptr, C2, n.g, n.b, out.p, x.NF, x.H * x.W, cfg.norm_groups, n.eps, silu ? 1 : 0, stats, st),
+         "groupnorm");
+    });
     return out;
   }
   // out = LN(x (+ pre_add per batch item)) (+ pe per frame); returns the normalised tensor, x_new receives x + pre_add
   Tens op_ln(const Tens& x, const Norm& n, const __half* pre_add, int64_t rows_per_b, Tens* x_new, const __half* pe, int F) {
     Tens out = alloc_act(x.NF, x.H, x.W, x.C);
     if (pre_add && x_new) *x_new = alloc_act(x.NF, x.H, x.W, x.C);
-    if (ar.dry) return out;
-    launches += 1;
-    Timed tm(this, CAT_NORM, 0, "layernorm", x.rows(), x.C, 0);
-    ck(launch_layernorm(x.p, n.g, n.b, out.p, x.rows(), x.C, n.eps, pre_add, rows_per_b, (pre_add && x_new) ? x_new->p : nullptr, pe, x.H * x.W, F, st),
-       "layernorm");
+    launch(1, {CAT_NORM, "layernorm", 0, x.rows(), x.C, 0}, [&] {
+      ck(launch_layernorm(x.p, n.g, n.b, out.p, x.rows(), x.C, n.eps, pre_add, rows_per_b, (pre_add && x_new) ? x_new->p : nullptr, pe, x.H * x.W, F, st),
+         "layernorm");
+    });
     return out;
   }
   void gemm(const __half* A, int64_t lda, const __half* A2, int64_t lda2, int64_t K1, const Mat& w, __half* out, int64_t ldc, int64_t M,
             const hv_epilogue* ep) {
-    if (ar.dry) return;
-    launches += 1;
-    Timed tm(this, CAT_GEMM, 2.0 * M * w.rows * w.cols, (ep && ep->geglu) ? "gemm_geglu" : ((ep && ep->residual) ? "gemm_res" : "gemm"), M, w.rows, w.cols);
-    ckop(op_gemm(A, lda, A2, lda2, K1, w.p, out, ldc, M, w.rows, w.cols, ep, st), "gemm");
+    const char* label = (ep && ep->geglu) ? "gemm_geglu" : ((ep && ep->residual) ? "gemm_res" : "gemm");
+    launch(1, {CAT_GEMM, label, 2.0 * M * w.rows * w.cols, M, w.rows, w.cols},
+           [&] { ckop(op_gemm(A, lda, A2, lda2, K1, w.p, out, ldc, M, w.rows, w.cols, ep, st), "gemm"); });
   }
   // y = x W^T + b (+ residual)
   Tens op_linear(const Tens& x, const Lin& l, const Tens* residual, int act = HV_ACT_NONE, bool geglu = false) {
@@ -596,7 +594,6 @@ struct hv_model {
     if (x.C != c.cin_pad) fail(HV_ERR_INVALID, "conv3x3: input has %d channels, weight packed for %d", x.C, c.cin_pad);
     const int Ho = stride == 1 ? x.H : x.H / 2, Wo = stride == 1 ? x.W : x.W / 2;
     Tens out = alloc_act(x.NF, Ho, Wo, c.cout_pad);
-    if (ar.dry) return out;
     hv_epilogue ep{};
     ep.bias = c.bias;
     ep.rowvec = rowvec;
@@ -604,17 +601,15 @@ struct hv_model {
     ep.rows_per_group = static_cast<int32_t>(rows_per_group);
     ep.act = act;
     if (residual) { ep.residual = residual->p; ep.ldr = residual->C; }
-    launches += 1;
-    Timed tm(this, CAT_CONV, 2.0 * out.rows() * c.cout * 9.0 * c.cin, stride == 1 ? "conv3" : "conv3_s2", out.rows(), c.cout_pad, 9LL * c.cin_pad);
-    ckop(op_conv3x3(x.p, c.w.p, out.p, c.cout_pad, x.NF, x.H, x.W, c.cin_pad, c.cout_pad, stride, &ep, st), "conv3x3");
+    launch(1, {CAT_CONV, stride == 1 ? "conv3" : "conv3_s2", 2.0 * out.rows() * c.cout * 9.0 * c.cin, out.rows(), c.cout_pad, 9LL * c.cin_pad},
+           [&] { ckop(op_conv3x3(x.p, c.w.p, out.p, c.cout_pad, x.NF, x.H, x.W, c.cin_pad, c.cout_pad, stride, &ep, st), "conv3x3"); });
     return out;
   }
   __half* op_small_linear(const __half* x, const Lin& l, int M, int act_in) {
     __half* out = alloc_h(static_cast<int64_t>(M) * l.w.rows);
-    if (ar.dry) return out;
-    launches += 1;
-    Timed tm(this, CAT_MISC, 2.0 * M * l.w.rows * l.w.cols);
-    ck(launch_small_linear(x, l.w.p, l.bias, out, M, static_cast<int>(l.w.rows), static_cast<int>(l.w.cols), act_in, st), "small_linear");
+    launch(1, {CAT_MISC, "", 2.0 * M * l.w.rows * l.w.cols}, [&] {
+      ck(launch_small_linear(x, l.w.p, l.bias, out, M, static_cast<int>(l.w.rows), static_cast<int>(l.w.cols), act_in, st), "small_linear");
+    });
     return out;
   }
 
@@ -642,15 +637,12 @@ struct hv_model {
       fail(HV_ERR_INVALID, "resnet with concatenated input must have a shortcut conv");
     }
     // conv2 + bias, + residual, written straight into `out`
-    if (!ar.dry) {
-      hv_epilogue ep{};
-      ep.bias = r.c2.bias;
-      ep.residual = res.p;
-      ep.ldr = res.C;
-      launches += 1;
-      Timed tm(this, CAT_CONV, 2.0 * x.rows() * r.cout * 9.0 * r.cout, "conv3_res", x.rows(), r.cout, 9LL * r.c2.cin_pad);
-      ckop(op_conv3x3(h2.p, r.c2.w.p, out.p, r.cout, x.NF, x.H, x.W, r.c2.cin_pad, r.c2.cout_pad, 1, &ep, st), "resnet conv2");
-    }
+    hv_epilogue ep{};
+    ep.bias = r.c2.bias;
+    ep.residual = res.p;
+    ep.ldr = res.C;
+    launch(1, {CAT_CONV, "conv3_res", 2.0 * x.rows() * r.cout * 9.0 * r.cout, x.rows(), r.cout, 9LL * r.c2.cin_pad},
+           [&] { ckop(op_conv3x3(h2.p, r.c2.w.p, out.p, r.cout, x.NF, x.H, x.W, r.c2.cin_pad, r.c2.cout_pad, 1, &ep, st), "resnet conv2"); });
     return out;
   }
 
@@ -674,15 +666,13 @@ struct hv_model {
       const int64_t vrows = static_cast<int64_t>(w.heads) * w.dv;
       __half* vt = alloc_h(vrows * ldvt);
       // V^T[C][frame n: n*Lp + j] = Wv [C][C] * n1^T : weights are the "A" operand, activations the batched "B" operand
-      if (!ar.dry) {
-        launches += 1;
-        Timed tm(this, CAT_GEMM, 2.0 * tokens * C * C, "gemm_vt", vrows, tokens, C);
-        ckop(op_gemm_batched_b(w.wv.p, C, n1.p, C, vt, ldvt, vrows, x.NF, L, Lp, C, w.vones, st), "V^T gemm");
-      }
+      launch(1, {CAT_GEMM, "gemm_vt", 2.0 * tokens * C * C, vrows, tokens, C},
+             [&] { ckop(op_gemm_batched_b(w.wv.p, C, n1.p, C, vt, ldvt, vrows, x.NF, L, Lp, C, w.vones, st), "V^T gemm"); });
       // write hook (mutual_self_attention.py:137-146): the bank IS LayerNorm-1's output; attention then runs on itself only
-      if (bank_out != nullptr && !ar.dry) {
-        launches += 1;
-        ck(cudaMemcpyAsync(bank_out[w.reader_idx], n1.p, static_cast<size_t>(tokens) * C * 2, cudaMemcpyDeviceToDevice, st), "bank write");
+      if (bank_out != nullptr) {
+        launch(1, {}, [&] {
+          ck(cudaMemcpyAsync(bank_out[w.reader_idx], n1.p, static_cast<size_t>(tokens) * C * 2, cudaMemcpyDeviceToDevice, st), "bank write");
+        });
       }
       // HV_FLAG_CFG: batch = [uncond ; cond], the first half ignores the bank.  HV_FLAG_UNCOND_ONLY / HV_FLAG_COND_ONLY: the batch
       // holds one CFG half only (a (window x CFG-half) unit of a multi-GPU split); a cond-only batch of B items reads the LAST B
@@ -706,27 +696,23 @@ struct hv_model {
         Lbp = rup(w.bank_L, 8);
         ldvbt = static_cast<int64_t>(B) * Lbp;
         vbt = alloc_h(vrows * ldvbt);
-        if (!ar.dry) {
-          launches += 1;
-          Timed tm(this, CAT_GEMM, 2.0 * bt * C * C);
-          ckop(op_gemm_batched_b(w.wv.p, C, bank, C, vbt, ldvbt, vrows, B, w.bank_L, Lbp, C, w.vones, st), "bank V^T gemm");
-        }
+        // its profile row has no label and no shape, so bench.py's per-shape GEMM roofline (gemm_classes) leaves it out
+        launch(1, {CAT_GEMM, "", 2.0 * bt * C * C},
+               [&] { ckop(op_gemm_batched_b(w.wv.p, C, bank, C, vbt, ldvbt, vrows, B, w.bank_L, Lbp, C, w.vones, st), "bank V^T gemm"); });
       }
       Tens o = alloc_act(x.NF, x.H, x.W, C);
-      if (!ar.dry) {
+      const int Lb = use_bank ? static_cast<int>(w.bank_L) : 0, nf_nobank = cfg_split ? (B / 2) * F : 0;
+      launch(1, {CAT_ATTN, "attn", 4.0 * L * w.C * (static_cast<double>(x.NF) * L + static_cast<double>(x.NF - nf_nobank) * Lb), x.NF, L, w.d}, [&] {
         AttnArgs a{};
         a.q = qk; a.k = qk + hp; a.vt = vt; a.out = o.p;
         a.NF = x.NF; a.L = L; a.heads = w.heads; a.d = w.d; a.dpad = w.dpad;
         a.ldq = 2 * hp; a.ldk = 2 * hp; a.ldvt = ldvt; a.ldo = C;
-        a.kb = kb; a.vbt = vbt; a.Lb = use_bank ? static_cast<int>(w.bank_L) : 0; a.ldkb = hp; a.ldvbt = ldvbt;
-        a.F = F; a.nf_nobank = cfg_split ? (B / 2) * F : 0;
+        a.kb = kb; a.vbt = vbt; a.Lb = Lb; a.ldkb = hp; a.ldvbt = ldvbt;
+        a.F = F; a.nf_nobank = nf_nobank;
         a.vt_stride = Lp; a.vbt_stride = Lbp;
-        launches += 1;
-        const double nb_frames = x.NF - a.nf_nobank;
-        Timed tm(this, CAT_ATTN, 4.0 * L * w.C * (static_cast<double>(x.NF) * L + nb_frames * a.Lb), "attn", x.NF, L, w.d);
         cudaError_t e = launch_attention(a, sms, st);
         if (e != cudaSuccess) fail(HV_ERR_CUDA, "attention (%s): %s %s", w.name.c_str(), cudaGetErrorString(e), tma_last_error());
-      }
+      });
       hv_epilogue ep{};
       ep.bias = w.out1.bias;
       ep.residual = t.p;
@@ -771,11 +757,8 @@ struct hv_model {
     __half* qkv = alloc_h(t.rows() * 3 * C);
     gemm(n.p, C, nullptr, 0, 0, a.wqkv, qkv, 3 * C, t.rows(), nullptr);
     Tens o = alloc_act(t.NF, t.H, t.W, C);
-    if (!ar.dry) {
-      launches += 1;
-      Timed tm(this, CAT_TATTN, 4.0 * t.rows() * F * C, "tattn", t.rows(), F, C);
-      ck(launch_temporal_attention(qkv, o.p, B, F, t.H * t.W, heads, d, st), "temporal attention");
-    }
+    launch(1, {CAT_TATTN, "tattn", 4.0 * t.rows() * F * C, t.rows(), F, C},
+           [&] { ck(launch_temporal_attention(qkv, o.p, B, F, t.H * t.W, heads, d, st), "temporal attention"); });
     hv_epilogue ep{};
     ep.bias = a.out.bias;
     ep.residual = t.p;
@@ -808,15 +791,16 @@ struct hv_model {
     ar.dry = dry;
     ar.off = 0;
     ar.peak = 0;
-    launches = 0;
     tap_list.clear();
-    if (!dry) { recs.clear(); ev_used = 0; }
     if (dry) {
       ar.base = nullptr;
       ar.cap = 0;
-    } else {
+    } else {   // a planning pass keeps the launch count and the profile of the last forward
       ar.base = static_cast<uint8_t*>(ws);
       ar.cap = ws_bytes;
+      launches = 0;
+      recs.clear();
+      ev_used = 0;
     }
   }
 
@@ -827,76 +811,66 @@ struct hv_model {
     if ((H % 8) || (W % 8)) fail(HV_ERR_INVALID, "latent size %dx%d must be a multiple of 8 (three stride-2 levels)", H, W);
     // time embedding (unet_3d.py:446-467)
     __half* tsin = alloc_h(static_cast<int64_t>(B) * ch[0]);
-    if (!ar.dry) { launches += 1; ck(launch_timestep_embedding(timestep, ts_table, ts_index, tsin, B, ch[0], st), "timestep embedding"); }
+    launch(1, {}, [&] { ck(launch_timestep_embedding(timestep, ts_table, ts_index, tsin, B, ch[0], st), "timestep embedding"); });
     __half* e1 = op_small_linear(tsin, te1, B, HV_ACT_NONE);
     __half* emb = op_small_linear(e1, te2, B, HV_ACT_SILU);
     // conv_in (+ pose_cond_fea as the epilogue residual); the 4 latent channels are zero-padded to one 64-wide k-block
     Tens x0 = alloc_act(NF, H, W, conv_in.cin_pad);
     Tens pc = pose ? alloc_act(NF, H, W, ch[0]) : Tens{};
-    if (!ar.dry) {
-      launches += 2 + (pose ? 1 : 0);
+    launch(2 + (pose ? 1 : 0), {}, [&] {
       ck(cudaMemsetAsync(x0.p, 0, static_cast<size_t>(x0.numel()) * 2, st), "memset");
       ck(launch_ncfhw_to_nhwc(sample, x0.p, B, cfg.in_channels, F, H, W, 0, st, x0.C), "sample layout");
       if (pose) ck(launch_ncfhw_to_nhwc(pose, pc.p, B, ch[0], F, H, W, 0, st), "pose layout");
-    }
+    });
     Tens h = op_conv3(x0, conv_in, 1, nullptr, 1, HV_ACT_NONE, pose ? &pc : nullptr);
     tap("conv_in", h);
+    // layer j of stage s (skip: the down-path tensor an up-path resnet concatenates)
+    auto layer = [&](const Stage& s, size_t j, const Tens* skip) {
+      const std::string sj = "." + std::to_string(j);
+      h = resnet_fwd(s.res[j], h, skip, emb, B, F);
+      tap(s.name + ".resnets" + sj, h);
+      if (j < s.attn.size()) { h = spatial_fwd(s.attn[j], h, ehs, B, F, flags); tap(s.name + ".attentions" + sj, h); }
+      if (j < s.mm.size()) { h = motion_fwd(s.mm[j], h, B, F); tap(s.name + ".motion_modules" + sj, h); }
+    };
     std::vector<Tens> skips{h};
-    for (size_t i = 0; i < down.size(); ++i) {
-      auto& d = down[i];
-      const std::string pb = "down_blocks." + std::to_string(i);
-      for (size_t j = 0; j < d.res.size(); ++j) {
-        h = resnet_fwd(d.res[j], h, nullptr, emb, B, F);
-        tap(pb + ".resnets." + std::to_string(j), h);
-        if (!d.attn.empty()) { h = spatial_fwd(d.attn[j], h, ehs, B, F, flags); tap(pb + ".attentions." + std::to_string(j), h); }
-        if (!d.mm.empty()) { h = motion_fwd(d.mm[j], h, B, F); tap(pb + ".motion_modules." + std::to_string(j), h); }
+    for (const Stage& s : down) {
+      for (size_t j = 0; j < s.res.size(); ++j) {
+        layer(s, j, nullptr);
         skips.push_back(h);
       }
-      if (d.has_down) {
-        h = op_conv3(h, d.down, 2, nullptr, 1, HV_ACT_NONE, nullptr);
-        tap(pb + ".downsamplers.0", h);
+      if (s.has_sampler) {
+        h = op_conv3(h, s.sampler, 2, nullptr, 1, HV_ACT_NONE, nullptr);
+        tap(s.name + ".downsamplers.0", h);
         skips.push_back(h);
       }
     }
-    h = resnet_fwd(mid.res[0], h, nullptr, emb, B, F);
-    tap("mid_block.resnets.0", h);
-    h = spatial_fwd(mid.attn[0], h, ehs, B, F, flags);
-    tap("mid_block.attentions.0", h);
-    if (!mid.mm.empty()) { h = motion_fwd(mid.mm[0], h, B, F); tap("mid_block.motion_modules.0", h); }
-    h = resnet_fwd(mid.res[1], h, nullptr, emb, B, F);
-    tap("mid_block.resnets.1", h);
-    for (size_t i = 0; i < up.size(); ++i) {
-      auto& u = up[i];
-      const std::string pb = "up_blocks." + std::to_string(i);
-      for (size_t j = 0; j < u.res.size(); ++j) {
-        Tens skip = skips.back();
+    layer(mid, 0, nullptr);
+    layer(mid, 1, nullptr);
+    for (const Stage& s : up) {
+      for (size_t j = 0; j < s.res.size(); ++j) {
+        const Tens skip = skips.back();
         skips.pop_back();
-        h = resnet_fwd(u.res[j], h, &skip, emb, B, F);
-        tap(pb + ".resnets." + std::to_string(j), h);
-        if (!u.attn.empty()) { h = spatial_fwd(u.attn[j], h, ehs, B, F, flags); tap(pb + ".attentions." + std::to_string(j), h); }
-        if (!u.mm.empty()) { h = motion_fwd(u.mm[j], h, B, F); tap(pb + ".motion_modules." + std::to_string(j), h); }
+        layer(s, j, &skip);
       }
-      if (u.has_up) {
+      if (s.has_sampler) {
         // Upsample3D (resnet.py:68-71): nearest 2x + 3x3 conv as four 2x2 convs of the source -- the 4x tensor is never materialised
-        Tens big = alloc_act(h.NF, 2 * h.H, 2 * h.W, u.up.cout);
-        if (!ar.dry) {
-          hv_epilogue ep{};
-          ep.bias = u.up.bias;
-          launches += 1;
-          Timed tm(this, CAT_CONV, 2.0 * big.rows() * u.up.cout * 4.0 * u.up.cin, "upconv2x2", big.rows(), u.up.cout, 4LL * u.up.cin);
-          ckop(op_upconv2x2(h.p, u.up.w.p, big.p, u.up.cout, h.NF, h.H, h.W, u.up.cin, u.up.cout, &ep, st), "upsampler conv");
-        }
+        const Conv3& c = s.sampler;
+        Tens big = alloc_act(h.NF, 2 * h.H, 2 * h.W, c.cout);
+        hv_epilogue ep{};
+        ep.bias = c.bias;
+        launch(1, {CAT_CONV, "upconv2x2", 2.0 * big.rows() * c.cout * 4.0 * c.cin, big.rows(), c.cout, 4LL * c.cin},
+               [&] { ckop(op_upconv2x2(h.p, c.w.p, big.p, c.cout, h.NF, h.H, h.W, c.cin, c.cout, &ep, st), "upsampler conv"); });
         h = big;
-        tap(pb + ".upsamplers.0", h);
+        tap(s.name + ".upsamplers.0", h);
       }
     }
     if (cfg.kind == HV_KIND_UNET2D_REF) {   // no post-process: the forward's value is the last up block's output (B, C0, h, w)
-      if (outp != nullptr && !ar.dry) { launches += 1; ck(launch_nhwc_to_ncfhw(h.p, h.C, outp, B, ch[0], F, H, W, st), "hidden layout"); }
+      if (outp != nullptr) launch(1, {}, [&] { ck(launch_nhwc_to_ncfhw(h.p, h.C, outp, B, ch[0], F, H, W, st), "hidden layout"); });
       return;
     }
     Tens hn = op_gn(h, nullptr, norm_out, true);
     Tens y = op_conv3(hn, conv_out, 1, nullptr, 1, HV_ACT_NONE, nullptr);
-    if (!ar.dry) { launches += 1; ck(launch_nhwc_to_ncfhw(y.p, y.C, outp, B, cfg.out_channels, F, H, W, st), "output layout"); }
+    launch(1, {}, [&] { ck(launch_nhwc_to_ncfhw(y.p, y.C, outp, B, cfg.out_channels, F, H, W, st), "output layout"); });
   }
 
   void pose_guider_forward(const __half* cond, __half* outp, int B, int F, int H, int W) {
@@ -906,20 +880,16 @@ struct hv_model {
     if (pg_fast_in) {
       // conv_in (3 -> 16) straight from the (B, 3, F, H, W) image: no layout pass, 16-channel output
       h = alloc_act(NF, H, W, pg_in.cout);
-      if (!ar.dry) {
-        launches += 1;
-        Timed tm(this, CAT_CONV, 2.0 * h.rows() * pg_in.cout * 9.0 * pg_in.cin, "pg_conv_in", h.rows(), pg_in.cout, 9LL * pg_in.cin);
-        ck(launch_pg_conv_in(cond, pg_in.w, pg_in.bias, h.p, B, F, H, W, HV_ACT_SILU, sms, st), "pose conv_in");
-      }
+      launch(1, {CAT_CONV, "pg_conv_in", 2.0 * h.rows() * pg_in.cout * 9.0 * pg_in.cin, h.rows(), pg_in.cout, 9LL * pg_in.cin},
+             [&] { ck(launch_pg_conv_in(cond, pg_in.w, pg_in.bias, h.p, B, F, H, W, HV_ACT_SILU, sms, st), "pose conv_in"); });
     } else {
       Tens x0 = alloc_act(NF, H, W, cfg.pg_cond_channels);
       h = alloc_act(NF, H, W, pg_convs[0].cin_pad);
-      if (!ar.dry) {
-        launches += 3;
+      launch(3, {}, [&] {
         ck(launch_ncfhw_to_nhwc(cond, x0.p, B, cfg.pg_cond_channels, F, H, W, 0, st), "pose image layout");
         ck(cudaMemsetAsync(h.p, 0, static_cast<size_t>(h.numel()) * 2, st), "memset");
         ck(launch_conv3x3_direct_padded(x0.p, pg_in.w, pg_in.bias, h.p, NF, H, W, pg_in.cin, pg_in.cout, h.C, HV_ACT_SILU, sms, st), "pose conv_in");
-      }
+      });
     }
     for (size_t i = 0; i < pg_convs.size(); ++i) {
       const bool last = i + 1 == pg_convs.size();
@@ -930,12 +900,9 @@ struct hv_model {
         const int Ho = pg_strides[i] == 1 ? h.H : h.H / 2, Wo = pg_strides[i] == 1 ? h.W : h.W / 2;
         if (h.C != c.cin) fail(HV_ERR_INVALID, "pose guider small conv %zu: input has %d channels, expects %d", i, h.C, c.cin);
         Tens out = alloc_act(NF, Ho, Wo, ld);
-        if (!ar.dry) {
-          if (ld > c.cout) { launches += 1; ck(cudaMemsetAsync(out.p, 0, static_cast<size_t>(out.numel()) * 2, st), "memset"); }
-          launches += 1;
-          Timed tm(this, CAT_CONV, 2.0 * out.rows() * c.cout * 9.0 * c.cin, pg_strides[i] == 1 ? "smallconv" : "smallconv_s2", out.rows(), c.cout, 9LL * c.cin);
-          ck(launch_smallconv(h.p, c.w.p, c.bias, out.p, NF, h.H, h.W, c.cin, c.cout, pg_strides[i], ld, HV_ACT_SILU, st), "pose small conv");
-        }
+        if (ld > c.cout) launch(1, {}, [&] { ck(cudaMemsetAsync(out.p, 0, static_cast<size_t>(out.numel()) * 2, st), "memset"); });
+        launch(1, {CAT_CONV, pg_strides[i] == 1 ? "smallconv" : "smallconv_s2", 2.0 * out.rows() * c.cout * 9.0 * c.cin, out.rows(), c.cout, 9LL * c.cin},
+               [&] { ck(launch_smallconv(h.p, c.w.p, c.bias, out.p, NF, h.H, h.W, c.cin, c.cout, pg_strides[i], ld, HV_ACT_SILU, st), "pose small conv"); });
         h = out;
         continue;
       }
@@ -943,7 +910,7 @@ struct hv_model {
       // the next conv expects cin_pad channels: cout_pad of this conv equals it by construction (both round to 64)
       if (!last && h.C != pg_convs[i + 1].cin_pad) fail(HV_ERR_INVALID, "pose guider channel padding mismatch at conv %zu", i);
     }
-    if (!ar.dry) { launches += 1; ck(launch_nhwc_to_ncfhw(h.p, h.C, outp, B, cfg.pg_out_channels, F, h.H, h.W, st), "pose output layout"); }
+    launch(1, {}, [&] { ck(launch_nhwc_to_ncfhw(h.p, h.C, outp, B, cfg.pg_out_channels, F, h.H, h.W, st), "pose output layout"); });
   }
 
   void camera_forward(const __half* plucker, __half* outp, int B, int F, int H, int W, const float* rays_K = nullptr, const float* rays_c2w = nullptr) {
@@ -951,15 +918,13 @@ struct hv_model {
     if ((H % r) || (W % r)) fail(HV_ERR_INVALID, "plucker map %dx%d must be a multiple of %d", H, W, r);
     const int cin0 = cfg.cam_cin / (r * r);
     Tens u = alloc_act(NF, H / r, W / r, cfg.cam_cin);
-    if (!ar.dry) {
-      launches += 1;
-      if (rays_K != nullptr) {   // SURVEY 8f-3: Plucker embedding generated in place of the unshuffle's gather
-        if (cin0 != 6) fail(HV_ERR_INVALID, "the Plucker producer makes 6 channels, encoder expects %d", cin0);
+    if (rays_K != nullptr && cin0 != 6) fail(HV_ERR_INVALID, "the Plucker producer makes 6 channels, encoder expects %d", cin0);
+    launch(1, {}, [&] {
+      if (rays_K != nullptr)   // SURVEY 8f-3: Plucker embedding generated in place of the unshuffle's gather
         ck(launch_plucker_unshuffle(rays_K, rays_c2w, u.p, NF, H, W, r, sms, st), "plucker unshuffle");
-      } else {
+      else
         ck(launch_pixel_unshuffle(plucker, u.p, B, cin0, F, H, W, r, sms, st), "pixel unshuffle");
-      }
-    }
+    });
     Tens x = op_conv3(u, cam_in, 1, nullptr, 1, HV_ACT_NONE, nullptr);
     for (int j = 0; j < cfg.cam_nums_rb; ++j) {
       // ResnetBlock (pose_adaptor.py:102-135, sk=True, ksize=1): x = block2(relu(block1(x))) + x
@@ -973,24 +938,27 @@ struct hv_model {
       x = op_linear(ffh, m.ff2, &t);
     }
     Tens z = op_linear(x, cam_zero, nullptr);
-    if (!ar.dry) { launches += 1; ck(launch_nhwc_to_ncfhw(z.p, z.C, outp, NF, C, 1, z.H, z.W, st), "camera output layout"); }
+    launch(1, {}, [&] { ck(launch_nhwc_to_ncfhw(z.p, z.C, outp, NF, C, 1, z.H, z.W, st), "camera output layout"); });
   }
 };
 
 // ------------------------------------------------------------------------------------------ C ABI
-#define HV_GUARD(h, ...)                                  \
-  try {                                                   \
-    __VA_ARGS__;                                          \
-    return HV_OK;                                         \
-  } catch (const Err& e) {                                \
-    if (h) (h)->err = e.msg;                              \
-    set_error("%s", e.msg.c_str());                       \
-    return e.code;                                        \
-  } catch (const std::exception& e) {                     \
-    if (h) (h)->err = e.what();                           \
-    set_error("%s", e.what());                            \
-    return HV_ERR_INVALID;                                \
+// Runs fn and turns an exception into its status; the message goes to hv_last_error(h) and to the library's last error.
+template <class Fn>
+static int guard(hv_model* h, Fn&& fn) {
+  try {
+    fn();
+    return HV_OK;
+  } catch (const Err& e) {
+    if (h) h->err = e.msg;
+    set_error("%s", e.msg.c_str());
+    return e.code;
+  } catch (const std::exception& e) {
+    if (h) h->err = e.what();
+    set_error("%s", e.what());
+    return HV_ERR_INVALID;
   }
+}
 
 // The forwards never allocate: a caller that passes no workspace must have called hv_reserve_workspace for a shape at least as
 // large (cudaMalloc synchronises the device and is illegal under stream capture).
@@ -1004,6 +972,32 @@ static void* get_ws(hv_model* m, void* ws, size_t ws_bytes, size_t need, size_t*
          m->private_ws_bytes, need);
   *have = m->private_ws_bytes;
   return m->private_ws;
+}
+
+// The planning pass: returns the workspace one forward needs at this shape and leaves the plan of its taps in tap_list.
+static size_t measure(hv_model* h, int B, int F, int H, int W, uint32_t flags = HV_FLAG_CFG) {
+  h->begin(nullptr, 0, true, nullptr);
+  if (h->cfg.kind == HV_KIND_UNET3D || h->cfg.kind == HV_KIND_UNET2D_REF) {
+    static __half dummy;
+    h->unet_forward(&dummy, 0, &dummy, h->cfg.kind == HV_KIND_UNET3D ? &dummy : nullptr, &dummy, B, F, H, W, flags);
+  } else if (h->cfg.kind == HV_KIND_POSE_GUIDER) {
+    h->pose_guider_forward(nullptr, nullptr, B, F, H, W);
+  } else {
+    h->camera_forward(nullptr, nullptr, B, F, H, W);
+  }
+  return h->ar.peak + 4096;
+}
+
+// Plans the forward at this shape, binds the workspace and the stream, and runs fwd.
+template <class Fwd>
+static void run_forward(hv_model* h, int kind, const char* what, int B, int F, int H, int W, uint32_t flags, void* workspace, size_t ws_bytes,
+                        hv_stream_t stream, Fwd&& fwd) {
+  if (!h->finalized || h->cfg.kind != kind) fail(HV_ERR_STATE, "handle is not a finalized %s", what);
+  const size_t need = measure(h, B, F, H, W, flags);
+  size_t have = 0;
+  void* ws = get_ws(h, workspace, ws_bytes, need, &have);
+  h->begin(ws, have, false, static_cast<cudaStream_t>(stream));
+  fwd();
 }
 
 extern "C" {
@@ -1040,7 +1034,7 @@ int hv_set_profiling(hv_handle h, int32_t enable) {
 
 int hv_dump_profile(hv_handle h, const char* path) {
   if (!h || !path) return HV_ERR_INVALID;
-  HV_GUARD(h, {
+  return guard(h, [&] {
     FILE* f = fopen(path, "w");
     if (!f) fail(HV_ERR_INVALID, "cannot open %s", path);
     if (!h->recs.empty()) ck(cudaEventSynchronize(h->recs.back().b), "profile sync");
@@ -1057,7 +1051,7 @@ int hv_dump_profile(hv_handle h, const char* path) {
 
 int hv_get_profile(hv_handle h, double* ms, double* flops, int64_t* count, int32_t ncat) {
   if (!h || !ms || !flops || !count) return HV_ERR_INVALID;
-  HV_GUARD(h, {
+  return guard(h, [&] {
     for (int i = 0; i < ncat; ++i) { ms[i] = 0; flops[i] = 0; count[i] = 0; }
     if (!h->recs.empty()) ck(cudaEventSynchronize(h->recs.back().b), "profile sync");
     for (const auto& r : h->recs) {
@@ -1078,7 +1072,7 @@ __global__ void cast_f32_to_f16(const float* __restrict__ x, __half* __restrict_
 
 int hv_set_weight(hv_handle h, const char* key, const void* dev_ptr, const int64_t* shape, int32_t ndim, int32_t dtype, hv_stream_t stream) {
   if (!h || !key || !dev_ptr || ndim < 0 || ndim > 8) return HV_ERR_INVALID;
-  HV_GUARD(h, {
+  return guard(h, [&] {
     if (h->finalized) fail(HV_ERR_STATE, "hv_set_weight after hv_finalize");
     Raw r;
     r.shape.assign(shape, shape + ndim);
@@ -1104,8 +1098,8 @@ int hv_set_weight(hv_handle h, const char* key, const void* dev_ptr, const int64
 
 int hv_finalize(hv_handle h, hv_stream_t stream) {
   if (!h) return HV_ERR_INVALID;
-  HV_GUARD(h, {
-    if (h->finalized) return HV_OK;
+  return guard(h, [&] {
+    if (h->finalized) return;
     h->st = static_cast<cudaStream_t>(stream);
     if (h->cfg.kind == HV_KIND_UNET3D || h->cfg.kind == HV_KIND_UNET2D_REF) h->build_unet();
     else if (h->cfg.kind == HV_KIND_POSE_GUIDER) h->build_pose_guider();
@@ -1121,7 +1115,7 @@ int hv_ref_block_dim(hv_handle h, int32_t i) {
 
 int hv_set_ref_bank(hv_handle h, int32_t idx, const void* dev_ptr, int64_t B_ref, int64_t L, int64_t C, hv_stream_t stream) {
   if (!h) return HV_ERR_INVALID;
-  HV_GUARD(h, {
+  return guard(h, [&] {
     if (!h->finalized) fail(HV_ERR_STATE, "hv_set_ref_bank before hv_finalize");
     if (idx < 0 || idx >= static_cast<int>(h->readers.size())) fail(HV_ERR_INVALID, "bank index %d out of range", idx);
     SpatialW* w = h->readers[idx];
@@ -1147,22 +1141,9 @@ int hv_clear_ref_banks(hv_handle h) {
   return HV_OK;
 }
 
-static size_t measure(hv_model* h, int B, int F, int H, int W, uint32_t flags = HV_FLAG_CFG) {
-  h->begin(nullptr, 0, true, nullptr);
-  if (h->cfg.kind == HV_KIND_UNET3D || h->cfg.kind == HV_KIND_UNET2D_REF) {
-    static __half dummy;
-    h->unet_forward(&dummy, 0, &dummy, h->cfg.kind == HV_KIND_UNET3D ? &dummy : nullptr, &dummy, B, F, H, W, flags);
-  } else if (h->cfg.kind == HV_KIND_POSE_GUIDER) {
-    h->pose_guider_forward(nullptr, nullptr, B, F, H, W);
-  } else {
-    h->camera_forward(nullptr, nullptr, B, F, H, W);
-  }
-  return h->ar.peak + 4096;
-}
-
 int hv_reserve_workspace(hv_handle h, int32_t B, int32_t F, int32_t height, int32_t width) {
   if (!h) return HV_ERR_INVALID;
-  HV_GUARD(h, {
+  return guard(h, [&] {
     if (!h->finalized) fail(HV_ERR_STATE, "hv_reserve_workspace before hv_finalize");
     const size_t need = measure(h, B, F, height, width);
     if (h->private_ws_bytes < need) {
@@ -1184,13 +1165,8 @@ int hv_set_timestep_source(hv_handle h, const int64_t* dev_table, const int32_t*
 
 int hv_debug_tap_count(hv_handle h, int32_t B, int32_t F, int32_t height, int32_t width) {
   if (!h || !h->finalized) return HV_ERR_INVALID;
-  try {
-    measure(h, B, F, height, width);
-    return static_cast<int>(h->tap_list.size());
-  } catch (const Err& e) {
-    h->err = e.msg;
-    return e.code;
-  }
+  const int status = guard(h, [&] { measure(h, B, F, height, width); });
+  return status == HV_OK ? static_cast<int>(h->tap_list.size()) : status;
 }
 
 int hv_debug_tap_info(hv_handle h, int32_t i, char* name, int32_t name_cap, int64_t* dims4) {
@@ -1209,89 +1185,65 @@ int hv_debug_set_taps(hv_handle h, void* const* dst, int32_t n) {
 
 size_t hv_workspace_bytes(hv_handle h, int32_t B, int32_t F, int32_t height, int32_t width) {
   if (!h || !h->finalized) return 0;
-  try {
-    return measure(h, B, F, height, width);
-  } catch (const Err& e) {
-    h->err = e.msg;
-    return 0;
-  }
+  size_t need = 0;
+  return guard(h, [&] { need = measure(h, B, F, height, width); }) == HV_OK ? need : 0;
 }
 
 int hv_unet3d_forward(hv_handle h, const void* sample, int64_t timestep, const void* ehs, const void* pose, void* out, int32_t B, int32_t F,
                       int32_t height, int32_t width, uint32_t flags, void* workspace, size_t ws_bytes, hv_stream_t stream) {
   if (!h || !sample || !ehs || !out) return HV_ERR_INVALID;
-  HV_GUARD(h, {
-    if (!h->finalized || h->cfg.kind != HV_KIND_UNET3D) fail(HV_ERR_STATE, "handle is not a finalized UNet3D");
+  return guard(h, [&] {
     if ((flags & HV_FLAG_UNCOND_ONLY) && (flags & HV_FLAG_COND_ONLY)) fail(HV_ERR_INVALID, "HV_FLAG_UNCOND_ONLY and HV_FLAG_COND_ONLY are exclusive");
-    const size_t need = measure(h, B, F, height, width, flags);
-    size_t have = 0;
-    void* ws = get_ws(h, workspace, ws_bytes, need, &have);
-    h->begin(ws, have, false, static_cast<cudaStream_t>(stream));
-    h->unet_forward(static_cast<const __half*>(sample), timestep, static_cast<const __half*>(ehs), static_cast<const __half*>(pose),
-                    static_cast<__half*>(out), B, F, height, width, flags);
+    run_forward(h, HV_KIND_UNET3D, "UNet3D", B, F, height, width, flags, workspace, ws_bytes, stream, [&] {
+      h->unet_forward(static_cast<const __half*>(sample), timestep, static_cast<const __half*>(ehs), static_cast<const __half*>(pose),
+                      static_cast<__half*>(out), B, F, height, width, flags);
+    });
   });
 }
 
 int hv_unet2d_reference_forward(hv_handle h, const void* sample, int64_t timestep, const void* ehs, void* hidden_out, void* const* bank_out,
                                 int32_t n_banks, int32_t B, int32_t height, int32_t width, void* workspace, size_t ws_bytes, hv_stream_t stream) {
   if (!h || !sample || !ehs || !bank_out) return HV_ERR_INVALID;
-  HV_GUARD(h, {
-    if (!h->finalized || h->cfg.kind != HV_KIND_UNET2D_REF) fail(HV_ERR_STATE, "handle is not a finalized reference (writer) UNet2D");
-    if (n_banks != static_cast<int>(h->readers.size())) fail(HV_ERR_INVALID, "expected %d bank destinations, got %d", (int)h->readers.size(), n_banks);
-    for (int i = 0; i < n_banks; ++i)
-      if (bank_out[i] == nullptr) fail(HV_ERR_INVALID, "bank destination %d is NULL", i);
-    const size_t need = measure(h, B, 1, height, width);
-    size_t have = 0;
-    void* ws = get_ws(h, workspace, ws_bytes, need, &have);
-    h->begin(ws, have, false, static_cast<cudaStream_t>(stream));
-    h->bank_out = reinterpret_cast<__half* const*>(bank_out);
-    try {
+  return guard(h, [&] {
+    run_forward(h, HV_KIND_UNET2D_REF, "reference (writer) UNet2D", B, 1, height, width, HV_FLAG_CFG, workspace, ws_bytes, stream, [&] {
+      if (n_banks != static_cast<int>(h->readers.size())) fail(HV_ERR_INVALID, "expected %d bank destinations, got %d", (int)h->readers.size(), n_banks);
+      for (int i = 0; i < n_banks; ++i)
+        if (bank_out[i] == nullptr) fail(HV_ERR_INVALID, "bank destination %d is NULL", i);
+      struct BankOut {   // the bank destinations belong to this forward only
+        hv_model* m;
+        ~BankOut() { m->bank_out = nullptr; }
+      } reset{h};
+      h->bank_out = reinterpret_cast<__half* const*>(bank_out);
       h->unet_forward(static_cast<const __half*>(sample), timestep, static_cast<const __half*>(ehs), nullptr, static_cast<__half*>(hidden_out), B, 1,
                       height, width, 0);
-    } catch (...) {
-      h->bank_out = nullptr;
-      throw;
-    }
-    h->bank_out = nullptr;
+    });
   });
 }
 
 int hv_pose_guider_forward(hv_handle h, const void* cond, void* out, int32_t B, int32_t F, int32_t H, int32_t W, void* workspace,
                            size_t ws_bytes, hv_stream_t stream) {
   if (!h || !cond || !out) return HV_ERR_INVALID;
-  HV_GUARD(h, {
-    if (!h->finalized || h->cfg.kind != HV_KIND_POSE_GUIDER) fail(HV_ERR_STATE, "handle is not a finalized PoseGuider");
-    const size_t need = measure(h, B, F, H, W);
-    size_t have = 0;
-    void* ws = get_ws(h, workspace, ws_bytes, need, &have);
-    h->begin(ws, have, false, static_cast<cudaStream_t>(stream));
-    h->pose_guider_forward(static_cast<const __half*>(cond), static_cast<__half*>(out), B, F, H, W);
+  return guard(h, [&] {
+    run_forward(h, HV_KIND_POSE_GUIDER, "PoseGuider", B, F, H, W, HV_FLAG_CFG, workspace, ws_bytes, stream,
+                [&] { h->pose_guider_forward(static_cast<const __half*>(cond), static_cast<__half*>(out), B, F, H, W); });
   });
 }
 
 int hv_camera_encoder_forward(hv_handle h, const void* plucker, void* out, int32_t B, int32_t F, int32_t H, int32_t W, void* workspace,
                               size_t ws_bytes, hv_stream_t stream) {
   if (!h || !plucker || !out) return HV_ERR_INVALID;
-  HV_GUARD(h, {
-    if (!h->finalized || h->cfg.kind != HV_KIND_CAMERA_ENCODER) fail(HV_ERR_STATE, "handle is not a finalized CameraPoseEncoder");
-    const size_t need = measure(h, B, F, H, W);
-    size_t have = 0;
-    void* ws = get_ws(h, workspace, ws_bytes, need, &have);
-    h->begin(ws, have, false, static_cast<cudaStream_t>(stream));
-    h->camera_forward(static_cast<const __half*>(plucker), static_cast<__half*>(out), B, F, H, W);
+  return guard(h, [&] {
+    run_forward(h, HV_KIND_CAMERA_ENCODER, "CameraPoseEncoder", B, F, H, W, HV_FLAG_CFG, workspace, ws_bytes, stream,
+                [&] { h->camera_forward(static_cast<const __half*>(plucker), static_cast<__half*>(out), B, F, H, W); });
   });
 }
 
 int hv_camera_encoder_forward_rays(hv_handle h, const float* intrinsics, const float* c2w, void* out, int32_t B, int32_t F, int32_t H, int32_t W,
                                    void* workspace, size_t ws_bytes, hv_stream_t stream) {
   if (!h || !intrinsics || !c2w || !out) return HV_ERR_INVALID;
-  HV_GUARD(h, {
-    if (!h->finalized || h->cfg.kind != HV_KIND_CAMERA_ENCODER) fail(HV_ERR_STATE, "handle is not a finalized CameraPoseEncoder");
-    const size_t need = measure(h, B, F, H, W);
-    size_t have = 0;
-    void* ws = get_ws(h, workspace, ws_bytes, need, &have);
-    h->begin(ws, have, false, static_cast<cudaStream_t>(stream));
-    h->camera_forward(nullptr, static_cast<__half*>(out), B, F, H, W, intrinsics, c2w);
+  return guard(h, [&] {
+    run_forward(h, HV_KIND_CAMERA_ENCODER, "CameraPoseEncoder", B, F, H, W, HV_FLAG_CFG, workspace, ws_bytes, stream,
+                [&] { h->camera_forward(nullptr, static_cast<__half*>(out), B, F, H, W, intrinsics, c2w); });
   });
 }
 

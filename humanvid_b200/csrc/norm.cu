@@ -6,7 +6,6 @@
 #include <stdlib.h>
 
 #include "ptx.cuh"
-#include "tuning.h"
 
 namespace hv {
 
@@ -269,9 +268,7 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const __half* __restrict
 // the batch: a forward of one CFG half (a unit of the multi-GPU split) is then bitwise equal to that half of a CFG batch.
 // (Measured and rejected: normalising ~56 MB chunks of frames at a time so that the apply pass re-reads from L2 what the statistics pass
 // just pulled in -- the smaller launches lose far more bandwidth than the L2 hits return: 135 us -> 250 us at level 0.)
-static void gn_plan(int C, int NF, int HW, int num_sms, int* threads, int* slabs, int* rows_per_block) {
-  (void)NF;
-  (void)num_sms;
+static void gn_plan(int C, int HW, int* threads, int* slabs, int* rows_per_block) {
   const int vecs = C / 8;
   int t = vecs * (vecs >= 256 ? 1 : 256 / vecs);
   if (t > 1024) t = vecs;
@@ -283,23 +280,20 @@ static void gn_plan(int C, int NF, int HW, int num_sms, int* threads, int* slabs
   *slabs = sl;
   *rows_per_block = rpb;
 }
-size_t groupnorm_scratch_floats(int C, int NF, int HW, int groups, int num_sms) {
+size_t groupnorm_scratch_floats(int C, int NF, int HW, int groups) {
   int t, sl, rpb;
-  gn_plan(C, NF, HW, num_sms, &t, &sl, &rpb);
+  gn_plan(C, HW, &t, &sl, &rpb);
   return static_cast<size_t>(2) * NF * groups * (1 + sl);
 }
 
-int groupnorm_num_launches(int, int, int, int) { return 2; }
-
 cudaError_t launch_groupnorm(const __half* x1, int C1, const __half* x2, int C2, const __half* gamma, const __half* beta,
-                             __half* out, int NF, int HW, int groups, float eps, int silu, float* stats, int num_sms,
-                             cudaStream_t stream) {
+                             __half* out, int NF, int HW, int groups, float eps, int silu, float* stats, cudaStream_t stream) {
   const int C = C1 + C2;
   if (C % 8 || C1 % 8 || C % groups || ((C / groups) & 1) || groups > 32 * 8) return cudaErrorInvalidValue;
   const int vecs = C / 8;
   if (vecs > 1024) return cudaErrorInvalidValue;
   int threads, slabs, rows_per_block;
-  gn_plan(C, NF, HW, num_sms, &threads, &slabs, &rows_per_block);
+  gn_plan(C, HW, &threads, &slabs, &rows_per_block);
   if (threads < groups || threads < 32) return cudaErrorInvalidValue;
   float* partial = stats + static_cast<size_t>(2) * NF * groups;
   gn_stats_kernel<<<dim3(slabs, NF), threads, threads * 8 * sizeof(float), stream>>>(x1, C1, x2, C2, HW, groups, rows_per_block, partial);
@@ -321,11 +315,10 @@ cudaError_t launch_layernorm(const __half* x, const __half* gamma, const __half*
   const int lpr = vecs <= 40 ? 8 : (vecs <= 80 ? 16 : 32);
   const int wpb = 8;
   const long long warps = (rows + (32 / lpr) - 1) / (32 / lpr);
-  static const int ln_waves = static_cast<int>(tune_env("HV_LN_BLOCKS_PER_SM", 8));
   static int sms = 0;
   if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); }
   long long blocks = (warps + wpb - 1) / wpb;
-  if (ln_waves > 0 && blocks > static_cast<long long>(sms) * ln_waves) blocks = static_cast<long long>(sms) * ln_waves;
+  if (blocks > 8LL * sms) blocks = 8LL * sms;   // persistent grid: 8 blocks per SM
   const unsigned grid = static_cast<unsigned>(blocks);
   if (lpr == 8)
     layernorm_kernel<8><<<grid, wpb * 32, 0, stream>>>(x, gamma, beta, out, rows, C, eps, pre_add, rows_per_group, x_out, pe, hw, F);

@@ -8,7 +8,6 @@
 #include "gemm.cuh"
 #include "kernels.h"
 #include "tma.h"
-#include "tuning.h"
 
 namespace hv {
 
@@ -66,10 +65,6 @@ static void fill_epilogue(GemmEpilogue& e, const hv_epilogue* ep, __half* out, i
 // ties go to the wider tile (fewer A re-reads per output) unless that leaves SMs idle.
 static int pick_block_n(int64_t N, int64_t m_tiles, bool geglu, int sms) {
   if (geglu) return 256;
-  {
-    const int v = static_cast<int>(tune_env("HV_GEMM_BN", 0));  // tuning build only
-    if (v == 128 || v == 160 || v == 256) return v;
-  }
   const int cand[3] = {256, 160, 128};
   int best = 128;
   int64_t best_pad = -1;
@@ -153,6 +148,18 @@ int op_gemm_batched_b(const __half* A, int64_t lda, const __half* X, int64_t ldx
   return HV_OK;
 }
 
+// Tiling of an implicit-GEMM convolution over the NF x H x W grid of the pixels it computes: one M tile is a box of frames x rows x columns.
+static void set_conv_tiles(GemmProblem& p, int64_t NF, int64_t H, int64_t W) {
+  p.NF = static_cast<int>(NF);
+  p.H = static_cast<int>(H);
+  p.W = static_cast<int>(W);
+  choose_conv_box(p.NF, p.H, p.W, &p.bn, &p.bh, &p.bw);
+  p.tiles_n = (p.NF + p.bn - 1) / p.bn;
+  p.tiles_y = (p.H + p.bh - 1) / p.bh;
+  p.tiles_x = (p.W + p.bw - 1) / p.bw;
+  p.M = p.NF * p.H * p.W;
+}
+
 int op_conv3x3(const __half* X, const __half* Wp, __half* out, int64_t ldc, int64_t NF, int64_t H, int64_t W, int64_t Cin,
                int64_t Cout, int stride, const hv_epilogue* ep, cudaStream_t stream) {
   const int sms = device_sms();
@@ -169,19 +176,11 @@ int op_conv3x3(const __half* X, const __half* Wp, __half* out, int64_t ldc, int6
   p.cin_blocks = static_cast<int>(Cin / 64);
   p.cin = static_cast<int>(Cin);
   p.num_k_blocks = 9 * p.cin_blocks;
-  p.H = static_cast<int>(Ho);
-  p.W = static_cast<int>(Wo);
-  p.NF = static_cast<int>(NF);
-  const int bn_guess = pick_block_n(Cout, (static_cast<int64_t>(NF) * Ho * Wo + 127) / 128, false, sms);
-  choose_conv_box(p.NF, p.H, p.W, &p.bn, &p.bh, &p.bw);
-  p.tiles_n = (p.NF + p.bn - 1) / p.bn;
-  p.tiles_y = (p.H + p.bh - 1) / p.bh;
-  p.tiles_x = (p.W + p.bw - 1) / p.bw;
-  p.M = p.NF * p.H * p.W;
+  set_conv_tiles(p, NF, Ho, Wo);
+  const int bn = pick_block_n(Cout, (static_cast<int64_t>(NF) * Ho * Wo + 127) / 128, false, sms);
   CUtensorMap ma, mb;
   bool ok = stride == 1 ? make_map_nhwc(&ma, X, NF, H, W, Cin, p.bn, p.bh, p.bw) : make_map_nhwc_s2(&ma, X, NF, H, W, Cin, p.bn, p.bh, p.bw);
   if (!ok) { set_error("hv_op_conv3x3 X map: %s", tma_last_error()); return HV_ERR_TMA; }
-  const int bn = bn_guess;
   if (!make_map_2d(&mb, Wp, Cout, 9 * Cin, 9 * Cin, bn)) { set_error("hv_op_conv3x3 W map: %s", tma_last_error()); return HV_ERR_TMA; }
   GemmEpilogue e;
   fill_epilogue(e, ep, out, ldc, Cout);
@@ -207,18 +206,11 @@ int op_upconv2x2(const __half* X, const __half* Wp, __half* out, int64_t ldc, in
   p.cin_blocks = static_cast<int>(Cin / 64);
   p.cin = static_cast<int>(Cin);
   p.num_k_blocks = 4 * p.cin_blocks;
-  p.H = static_cast<int>(H);     // tile space = SOURCE pixels; the epilogue scatters to (2y + py, 2x + px)
-  p.W = static_cast<int>(W);
-  p.NF = static_cast<int>(NF);
+  set_conv_tiles(p, NF, H, W);   // tile space = SOURCE pixels; the epilogue scatters to (2y + py, 2x + px)
   p.b_par_rows = static_cast<int>(Cout);
   const int64_t rows = NF * H * W;
   const int bn = pick_block_n(Cout, (4 * rows + 127) / 128, false, sms);
   if (Cout % bn) { set_error("hv_op_upconv2x2: Cout=%lld must be a multiple of the %d-column tile", (long long)Cout, bn); return HV_ERR_INVALID; }
-  choose_conv_box(p.NF, p.H, p.W, &p.bn, &p.bh, &p.bw);
-  p.tiles_n = (p.NF + p.bn - 1) / p.bn;
-  p.tiles_y = (p.H + p.bh - 1) / p.bh;
-  p.tiles_x = (p.W + p.bw - 1) / p.bw;
-  p.M = p.NF * p.H * p.W;
   CUtensorMap ma, mb;
   if (!make_map_nhwc(&ma, X, NF, H, W, Cin, p.bn, p.bh, p.bw)) { set_error("hv_op_upconv2x2 X map: %s", tma_last_error()); return HV_ERR_TMA; }
   if (!make_map_2d(&mb, Wp, 4 * Cout, 4 * Cin, 4 * Cin, bn)) { set_error("hv_op_upconv2x2 W map: %s", tma_last_error()); return HV_ERR_TMA; }

@@ -127,7 +127,8 @@ int hv_debug_tap_count(hv_handle h, int32_t B, int32_t F, int32_t height, int32_
 int hv_debug_tap_info(hv_handle h, int32_t i, char* name, int32_t name_cap, int64_t* dims4);
 int hv_debug_set_taps(hv_handle h, void* const* dst, int32_t n);
 
-/* Kernel launches issued by the last forward on this handle (bench.py's gpu_launches). */
+/* Kernel launches issued by the last forward on this handle (bench.py's gpu_launches).  hv_workspace_bytes,
+ * hv_reserve_workspace and hv_debug_tap_count only plan a forward and leave it unchanged. */
 int64_t hv_last_launch_count(hv_handle h);
 
 /* Optional per-operator-category device timing of the next forwards (CUDA events around every launch on the caller's

@@ -133,8 +133,6 @@ int hv_op_ncfhw_to_nhwc(const void* X, void* out, int64_t B, int64_t C, int64_t 
                         hv_stream_t stream);
 int hv_op_nhwc_to_ncfhw(const void* X, int64_t ldx, void* out, int64_t B, int64_t C, int64_t F, int64_t H, int64_t W,
                         hv_stream_t stream);
-int hv_op_upsample2x(const void* X, void* out, int64_t NF, int64_t H, int64_t W, int64_t C, hv_stream_t stream);
-int hv_op_add(const void* A, const void* B, void* out, int64_t n, hv_stream_t stream);
 int hv_op_pixel_unshuffle(const void* X, void* out, int64_t B, int64_t C, int64_t F, int64_t H, int64_t W, int32_t r,
                           hv_stream_t stream);
 /* Plucker-embedding producer on the device (Camera + ray_condition, src/dataset/dance_image_h_v_camera.py:17-130; called from

@@ -330,7 +330,7 @@ def test_attention_with_reference_bank():
     assert attention_case(2, 9216, 8, 40, Lb=9216, Fr=1, nf_nobank=1, seed=92) < 1e-3
 
 
-def test_layout_roundtrip_and_glue():
+def test_layout_roundtrip_unshuffle_embedding_small_linear():
     B, Cc, Fr, H, W = 2, 4, 3, 16, 12
     x = dev(B, Cc, Fr, H, W, seed=100)
     nhwc = torch.zeros(B * Fr, H, W, 8, device="cuda", dtype=torch.half)
@@ -341,11 +341,7 @@ def test_layout_roundtrip_and_glue():
     back = torch.zeros_like(x)
     check(lib().hv_op_nhwc_to_ncfhw(ptr(nhwc), i64(8), ptr(back), i64(B), i64(Cc), i64(Fr), i64(H), i64(W), stream()))
     assert torch.equal(back, x)
-    y = dev(5, 6, 7, 64, seed=101)
-    up = torch.zeros(5, 12, 14, 64, device="cuda", dtype=torch.half)
-    check(lib().hv_op_upsample2x(ptr(y), ptr(up), i64(5), i64(6), i64(7), i64(64), stream()))
-    assert torch.equal(up, F.interpolate(y.permute(0, 3, 1, 2).float(), scale_factor=2.0, mode="nearest").permute(0, 2, 3, 1).half())
-    pl = dev(1, 6, 2, 16, 24, seed=102)
+    pl =dev(1, 6, 2, 16, 24, seed=102)
     un = torch.zeros(2, 2, 3, 384, device="cuda", dtype=torch.half)
     check(lib().hv_op_pixel_unshuffle(ptr(pl), ptr(un), i64(1), i64(6), i64(2), i64(16), i64(24), i32(8), stream()))
     ref = F.pixel_unshuffle(pl[0].permute(1, 0, 2, 3), 8).permute(0, 2, 3, 1)
