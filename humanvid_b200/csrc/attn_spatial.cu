@@ -10,6 +10,8 @@
 //                                  registers).  O stays in registers across key tiles; V^T carries a row of ones per head so
 //                                  O's extra column IS the softmax denominator (summed from the same fp16 P the MMA sees).
 //                                  O is rescaled only when a row max grows by more than 2^8 (lazy rescale).
+//                                  Pipelined by one key tile: S_{j+1} = Q K_{j+1} and O += P_j V_j are issued together and the
+//                                  softmax of S_{j+1} runs while P_j V_j is on the tensor cores (DESIGN.md section 3).
 // Keys come from two segments: the frame's own L tokens and, for frames of the conditional CFG half, the Lb tokens of
 // the batch item's reference bank -- the reference instead materialises cat([x, bank.repeat(F)]) per frame and
 // recomputes the unconditional half (mutual_self_attention.py:158-186).
@@ -50,7 +52,52 @@ struct ACfg {
   static constexpr int kStagesFit = (227 * 1024 - kQBytes - kMisc) / kStageBytes;
   static constexpr int kStages = kStagesFit > 4 ? 4 : kStagesFit;
   static constexpr int kSmemBytes = kQBytes + kStages * kStageBytes + kMisc;
+  // The one-tile software pipeline needs K_{j+1} resident while P_j V_j runs.  With a single stage (d = 160) K_{j+1} shares the
+  // slot of K_j and arrives late, and the pipelined loop measured 12 % slower than the serial one (H100 SXM, 400 W), so that case
+  // stays serial.
+  static constexpr bool kPipelined = kStages >= 2;
 };
+
+// Online softmax of one 64 x 128 score tile held in wgmma accumulator layout (thread row r = lane/4 (+8 for hh = 1), columns
+// 8 jj + 2 quad + e): row max across the four lanes of a row, the lazy-rescale decision (grow, alpha = 2^(m_old - m_new) for O),
+// then s <- 2^(s*scale - m) in place.  MASK sets keys >= kv_valid to -inf first.
+template <bool MASK>
+__device__ __forceinline__ void tile_softmax(float (&s)[KT / 2], int kv_valid, int quad, float sc, float (&m_used)[2], bool (&grow)[2],
+                                             float (&alpha)[2]) {
+  float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+  for (int jj = 0; jj < KT / 8; ++jj)
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const bool ok = !MASK || 8 * jj + 2 * quad + e < kv_valid;
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        float& v = s[4 * jj + 2 * hh + e];
+        if (MASK) v = ok ? v : -INFINITY;
+        mx[hh] = fmaxf(mx[hh], v);
+      }
+    }
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
+    mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
+    const float rowmax = mx[hh] * sc;
+    grow[hh] = rowmax > m_used[hh] + kRescaleThreshold;
+    if (grow[hh]) {
+      alpha[hh] = fast_exp2(m_used[hh] - rowmax);
+      m_used[hh] = rowmax;
+    }
+  }
+#pragma unroll
+  for (int jj = 0; jj < KT / 8; ++jj)
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        float& v = s[4 * jj + 2 * hh + e];
+        v = fast_exp2(fmaf(v, sc, -m_used[hh]));
+      }
+}
 
 struct AttnKernelArgs {
   __half* out;
@@ -143,82 +190,125 @@ attn_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ C
 #pragma unroll
   for (int i = 0; i < DV / 2; ++i) o[i] = 0.f;
   float m_used[2] = {-INFINITY, -INFINITY};
-  int stage = 0;
-  uint32_t phase = 0;
-  mbar_wait(bar_q, 0);
-  for (int j = 0; j < T; ++j) {
-    const bool self = j < Ts;
-    const int kv_valid = self ? min(KT, a.L - j * KT) : min(KT, a.Lb - (j - Ts) * KT);
-    // ---- S = Q K^T
-    float s[KT / 2];
-    mbar_wait(&bar_k_full[stage], phase);
-    const uint32_t aK = smem_u32(sKV + stage * C::kStageBytes);
-    wgmma_fence();
+  float s[KT / 2];          // scores of the next key tile, then its p = 2^(s*scale - m) in fp32
+  uint32_t pa[KT / 16][4];  // p of the current tile as the packed fp16 A fragments of O += P V (16 keys per fragment)
+  bool grow[2];
+  float alpha[2];
+
+  auto issue_qk = [&](int st) {
+    const uint32_t aK = smem_u32(sKV + st * C::kStageBytes);
 #pragma unroll
     for (int ks = 0; ks < DP / 16; ++ks)
       wgmma_ss<KT>(s, gmma_desc_k_sw128(aQ + (ks / 4) * QT * 128) + 2 * (ks % 4), gmma_desc_k_sw128(aK + (ks / 4) * KT * 128) + 2 * (ks % 4),
                    ks != 0 ? 1u : 0u);
     wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_fence_regs(s);
-    if (lane == 0) mbar_arrive(&bar_k_empty[stage]);
-
-    // ---- online softmax (keys past the segment's end are masked)
-    float mx[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-    for (int jj = 0; jj < KT / 8; ++jj)
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const bool ok = 8 * jj + 2 * quad + e < kv_valid;
-#pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-          float& v = s[4 * jj + 2 * hh + e];
-          v = ok ? v : -INFINITY;
-          mx[hh] = fmaxf(mx[hh], v);
-        }
-      }
-    float m_new[2];
+  };
+  // keys past the segment's end are masked; only a segment's last tile can be partial, every other tile skips the mask
+  auto softmax = [&](int j) {
+    const int kv_valid = j < Ts ? a.L - j * KT : a.Lb - (j - Ts) * KT;
+    if (kv_valid < KT)
+      tile_softmax<true>(s, kv_valid, quad, sc, m_used, grow, alpha);
+    else
+      tile_softmax<false>(s, KT, quad, sc, m_used, grow, alpha);
+  };
+  // Pipelined, O is rescaled branch-free (a factor of exactly 1 leaves O bit for bit as it was): ptxas serialises every wgmma of
+  // the kernel when a data-dependent branch writes O between two MMAs that accumulate into it.
+  auto rescale_o = [&] {
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
-      mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
-      mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
-      const float rowmax = mx[hh] * sc;
-      const bool grow = rowmax > m_used[hh] + kRescaleThreshold;
-      m_new[hh] = grow ? rowmax : m_used[hh];
-      if (grow) {
-        const float alpha = fast_exp2(m_used[hh] - m_new[hh]);
+      if (!C::kPipelined && !grow[hh]) continue;
+      const float f = grow[hh] ? alpha[hh] : 1.f;
 #pragma unroll
-        for (int jj = 0; jj < DV / 8; ++jj) {
-          o[4 * jj + 2 * hh] *= alpha;
-          o[4 * jj + 2 * hh + 1] *= alpha;
-        }
+      for (int jj = 0; jj < DV / 8; ++jj) {
+        o[4 * jj + 2 * hh] *= f;
+        o[4 * jj + 2 * hh + 1] *= f;
       }
-      m_used[hh] = m_new[hh];
     }
-    // p = 2^(s*scale - m) -> packed fp16 A fragments of the P V MMA (16 keys per fragment)
-    uint32_t pa[KT / 16][4];
+  };
+  auto pack_p = [&] {
 #pragma unroll
     for (int kk = 0; kk < KT / 16; ++kk)
 #pragma unroll
       for (int half = 0; half < 2; ++half)
 #pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-          const float* v = s + 4 * (2 * kk + half) + 2 * hh;
-          pa[kk][2 * half + hh] = pack_h2(fast_exp2(fmaf(v[0], sc, -m_used[hh])), fast_exp2(fmaf(v[1], sc, -m_used[hh])));
-        }
+        for (int hh = 0; hh < 2; ++hh) pa[kk][2 * half + hh] = pack_h2(s[4 * (2 * kk + half) + 2 * hh], s[4 * (2 * kk + half) + 2 * hh + 1]);
+  };
 
-    // ---- O += P V
-    mbar_wait(&bar_v_full[stage], phase);
-    const uint32_t aV = smem_u32(sKV + stage * C::kStageBytes + C::kKBytes);
-    wgmma_fence_regs(o);
-    wgmma_fence();
+  mbar_wait(bar_q, 0);
+  int stage = 0;
+  uint32_t phase = 0;
+  if constexpr (!C::kPipelined) {
+    // ---- one key tile at a time: S_j, softmax, O += P_j V_j
+    for (int j = 0; j < T; ++j) {
+      mbar_wait(&bar_k_full[stage], phase);
+      wgmma_fence();
+      issue_qk(stage);
+      wgmma_wait<0>();
+      wgmma_fence_regs(s);
+      if (lane == 0) mbar_arrive(&bar_k_empty[stage]);
+      softmax(j);
+      rescale_o();
+      pack_p();
+      mbar_wait(&bar_v_full[stage], phase);
+      const uint32_t aV = smem_u32(sKV + stage * C::kStageBytes + C::kKBytes);
+      wgmma_fence_regs(o);
+      wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < KT / 16; ++kk) wgmma_rs<DV>(o, pa[kk], gmma_desc_k_sw128(aV + (kk / 4) * C::kVChunk) + 2 * (kk % 4), 1u);
-    wgmma_commit();
+      for (int kk = 0; kk < KT / 16; ++kk) wgmma_rs<DV>(o, pa[kk], gmma_desc_k_sw128(aV + (kk / 4) * C::kVChunk) + 2 * (kk % 4), 1u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(o);
+      if (lane == 0) mbar_arrive(&bar_v_empty[stage]);
+      if (++stage == NS) { stage = 0; phase ^= 1; }
+    }
+  } else {
+    // ---- prologue: S_0, its softmax and P_0
+    mbar_wait(&bar_k_full[0], 0);
+    wgmma_fence();
+    issue_qk(0);
     wgmma_wait<0>();
-    wgmma_fence_regs(o);
-    if (lane == 0) mbar_arrive(&bar_v_empty[stage]);
-    if (++stage == NS) { stage = 0; phase ^= 1; }
+    wgmma_fence_regs(s);
+    if (lane == 0) mbar_arrive(&bar_k_empty[0]);
+    softmax(0);
+    rescale_o();
+    pack_p();
+
+    // ---- steady state, one key tile per iteration: S_{j+1} = Q K_{j+1} and O += P_j V_j are issued back to back; the softmax of
+    // S_{j+1} runs while P_j V_j is still on the tensor cores.  O is rescaled (and P_{j+1} written over P_j) once P_j V_j has completed,
+    // so O accumulates in the same order, with the same rescale decisions, as a strictly serial loop.
+    // `next`: tile j + 1 exists.  Called with a constant, so the last tile's copy has no conditional MMA issue (ptxas serialises
+    // wgmma behind any divergent path around one).
+    auto step = [&](int j, bool next) {
+      const int nstage = stage + 1 == NS ? 0 : stage + 1;
+      const uint32_t nphase = stage + 1 == NS ? phase ^ 1 : phase;
+      if (next) mbar_wait(&bar_k_full[nstage], nphase);
+      mbar_wait(&bar_v_full[stage], phase);
+      wgmma_fence_regs(o);
+      wgmma_fence();
+      if (next) issue_qk(nstage);
+      const uint32_t aV = smem_u32(sKV + stage * C::kStageBytes + C::kKBytes);
+#pragma unroll
+      for (int kk = 0; kk < KT / 16; ++kk) wgmma_rs<DV>(o, pa[kk], gmma_desc_k_sw128(aV + (kk / 4) * C::kVChunk) + 2 * (kk % 4), 1u);
+      wgmma_commit();
+      if (next) {
+        wgmma_wait<1>();
+        wgmma_fence_regs(s);
+        if (lane == 0) mbar_arrive(&bar_k_empty[nstage]);
+        softmax(j + 1);
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs(o);
+      wgmma_fence_regs(pa);
+      if (lane == 0) mbar_arrive(&bar_v_empty[stage]);
+      if (next) {
+        rescale_o();
+        pack_p();
+      }
+      stage = nstage;
+      phase = nphase;
+    };
+    for (int j = 0; j + 1 < T; ++j) step(j, true);
+    step(T - 1, false);
   }
 
   // ---- epilogue: O / denominator (column D of O, held by lane quad (D % 8) / 2 of the row)
@@ -242,8 +332,11 @@ cudaError_t launch_attn_t(const AttnArgs& a, cudaStream_t stream) {
   static_assert(C::kStages >= 1, "one K/V stage must fit in shared memory");
   CUtensorMap mq, mk, mvt, mkb, mvbt;
   const long long tokens = static_cast<long long>(a.NF) * a.L;
-  if (!make_map_2d(&mq, a.q, tokens, a.ldq, a.ldq, QT)) return cudaErrorInvalidValue;
-  if (!make_map_2d(&mk, a.k, tokens, a.ldk, a.ldk, KT)) return cudaErrorInvalidValue;
+  // the maps span the heads * dpad columns that exist: the last head's 64-column box then ends in TMA's zero fill instead of
+  // reading past the row (past the buffer's end for K's last token, where K sits after Q in an interleaved row)
+  const long long cols = static_cast<long long>(a.heads) * C::kDpad;
+  if (!make_map_2d(&mq, a.q, tokens, cols, a.ldq, QT)) return cudaErrorInvalidValue;
+  if (!make_map_2d(&mk, a.k, tokens, cols, a.ldk, KT)) return cudaErrorInvalidValue;
   if (!make_map_2d(&mvt, a.vt, static_cast<long long>(a.heads) * C::kDv, static_cast<long long>(a.NF) * a.vt_stride, a.ldvt, C::kDv)) return cudaErrorInvalidValue;
   mkb = mk;
   mvbt = mvt;
