@@ -37,6 +37,11 @@ int hv_op_conv3x3(const void* X, const void* Wp, void* out, int64_t ldc, int64_t
   return op_conv3x3(H(X), H(Wp), HM(out), ldc, NF, Hh, W, Cin, Cout, stride, ep, ST(stream));
 }
 
+int hv_op_conv3x3_s2_pad_end(const void* X, const void* Wp, void* out, int64_t ldc, int64_t NF, int64_t Hh, int64_t W, int64_t Cin, int64_t Cout,
+                             const hv_epilogue* ep, hv_stream_t stream) {
+  return op_conv3x3(H(X), H(Wp), HM(out), ldc, NF, Hh, W, Cin, Cout, 2, ep, ST(stream), true);
+}
+
 int hv_op_upconv2x2(const void* X, const void* Wp, void* out, int64_t ldc, int64_t NF, int64_t Hh, int64_t W, int64_t Cin, int64_t Cout,
                     const hv_epilogue* ep, hv_stream_t stream) {
   return op_upconv2x2(H(X), H(Wp), HM(out), ldc, NF, Hh, W, Cin, Cout, ep, ST(stream));
@@ -95,6 +100,20 @@ int hv_op_attention(const void* Q, const void* K, const void* Vt, void* out, int
   if ((ldq % 8) || (ldk % 8) || (ldvt % 8) || (ldo % 8) || (d % 8)) { set_error("hv_op_attention: strides / head dim must be multiples of 8"); return HV_ERR_INVALID; }
   cudaError_t e = launch_attention(a, device_sms(), ST(stream));
   if (e != cudaSuccess) { set_error("hv_op_attention: %s (%s)", cudaGetErrorString(e), tma_last_error()); return HV_ERR_CUDA; }
+  return HV_OK;
+}
+
+int hv_op_attention_d512(const void* Q, int64_t ldq, const void* K, int64_t ldk, const void* Vt, int64_t ldvt, int64_t vt_stride, void* out,
+                         int64_t ldo, int64_t NF, int64_t L, hv_stream_t stream) {
+  if (!device_sms()) return HV_ERR_CUDA;
+  if (!Q || !K || !Vt || !out || NF <= 0 || NF > 65535 || L <= 0 || L > (1 << 24) || (ldq % 8) || (ldk % 8) || (ldvt % 8) || (ldo % 8) ||
+      (vt_stride % 8) || vt_stride < L || ldq < 512 || ldk < 512 || ldo < 512) {
+    set_error("hv_op_attention_d512: bad shape NF=%lld L=%lld ldq=%lld ldk=%lld ldvt=%lld vt_stride=%lld ldo=%lld (strides multiples of 8, rows >= 512 wide, "
+              "vt_stride >= L)", (long long)NF, (long long)L, (long long)ldq, (long long)ldk, (long long)ldvt, (long long)vt_stride, (long long)ldo);
+    return HV_ERR_INVALID;
+  }
+  cudaError_t e = launch_attention_d512(H(Q), ldq, H(K), ldk, H(Vt), ldvt, vt_stride, HM(out), ldo, (int)NF, (int)L, ST(stream));
+  if (e != cudaSuccess) { set_error("hv_op_attention_d512: %s (%s)", cudaGetErrorString(e), tma_last_error()); return HV_ERR_CUDA; }
   return HV_OK;
 }
 

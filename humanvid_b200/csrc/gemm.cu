@@ -13,7 +13,8 @@
 // The A operand is addressed through TMA only, so a 3x3 convolution over a channels-last (N,H,W,C) tensor is the
 // same kernel: k-block kb = (tap, 64-channel block) and the tile of 128 output pixels is a (bn x bh x bw) box whose
 // input window is fetched with the box shifted by the tap offset; TMA's out-of-bounds zero fill is the padding.
-// Stride-2 convolutions view the same memory as (N, H/2, 2, W/2, 2*C) so each tap is again a dense box.
+// Stride-2 convolutions view the same memory as (N, H/2, 2, W/2, 2*C) so each tap is again a dense box; the end-padded
+// variant (pad (0, 1, 0, 1), padding 0) is the same view with every tap shifted by one input pixel.
 #include <cstdlib>
 
 #include "gemm.cuh"
@@ -150,10 +151,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ 
               // with the 3x3 taps that land on each pre-summed in the packed weight (tap = 2a + b)
               const int a = tap >> 1, b = tap & 1;
               tma_load_4d(sa, &map_a0, &bar_full[stage], cb * BLOCK_K, tc.x0 + b + tc.px - 1, tc.y0 + a + tc.py - 1, tc.n0);
-            } else {  // stride 2: memory viewed as (N, H/2, 2, W/2, 2C); input row 2*yo+dy-1, col 2*xo+dx-1
+            } else if (p.a_mode == A_CONV3X3_S2) {  // stride 2: memory viewed as (N, H/2, 2, W/2, 2C); input row 2*yo+dy-1, col 2*xo+dx-1
               const int ph = dy == 1 ? 0 : 1, pw = dx == 1 ? 0 : 1;
               tma_load_5d(sa, &map_a0, &bar_full[stage], pw * p.cin + cb * BLOCK_K, tc.x0 - (dx == 0 ? 1 : 0), ph,
                           tc.y0 - (dy == 0 ? 1 : 0), tc.n0);
+            } else {  // stride 2, padding at the end only: input row 2*yo+dy, col 2*xo+dx (the same view, the tap origin one pixel later)
+              const int ph = dy & 1, pw = dx & 1;
+              tma_load_5d(sa, &map_a0, &bar_full[stage], pw * p.cin + cb * BLOCK_K, tc.x0 + (dx >> 1), ph, tc.y0 + (dy >> 1), tc.n0);
             }
           }
           if (!BST) {

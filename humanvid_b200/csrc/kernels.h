@@ -23,6 +23,10 @@ struct AttnArgs {
   long long vt_stride, vbt_stride;       // columns between consecutive frames / bank items in V^T (multiples of 8)
 };
 cudaError_t launch_attention(const AttnArgs& a, int num_sms, cudaStream_t stream);
+// Single-head attention, d = 512 (AutoencoderKL mid block, attn_vae.cu): Q [NF*L][ldq], K [NF*L][ldk], V^T [512][ldvt] with frame n's
+// tokens at columns [n*vt_stride, n*vt_stride + L), out [NF*L][ldo]; scale 512^-1/2.
+cudaError_t launch_attention_d512(const __half* q, long long ldq, const __half* k, long long ldk, const __half* vt, long long ldvt, long long vt_stride,
+                                  __half* out, long long ldo, int NF, int L, cudaStream_t stream);
 
 cudaError_t launch_ncfhw_to_nhwc(const void* x, __half* out, int B, int C, int F, int H, int W, int src_fp32, cudaStream_t s, int ldo = 0);
 cudaError_t launch_nhwc_to_ncfhw(const __half* x, int ldx, __half* out, int B, int C, int F, int H, int W, cudaStream_t s);

@@ -1,6 +1,6 @@
 // Network runtime behind include/hv_b200.h: weight ingestion under the reference's state_dict keys, packing into
-// kernel layouts, a stack-allocated activation workspace, and the three forwards (UNet3DConditionModel, PoseGuider,
-// CameraPoseEncoder) expressed as sequences of the operators in ops.h / kernels.h.
+// kernel layouts, a stack-allocated activation workspace, and the forwards (UNet3DConditionModel, PoseGuider,
+// CameraPoseEncoder, AutoencoderKL encode / decode) expressed as sequences of the operators in ops.h / kernels.h.
 //
 // Activations are channels-last fp16 (N = B*F frames, H, W, C) == a [tokens][C] matrix, so the reference's
 // "b c f h w -> (b f) c h w", "(bf) c h w -> (bf) (hw) c" and "(b f) d c -> (b d) f c" rearranges never touch memory:
@@ -90,6 +90,7 @@ struct Tens {  // channels-last activation
 struct ResnetW {
   Norm n1, n2;
   Conv3 c1, c2;
+  bool has_temb = false;   // UNet resnets add time_emb_proj(silu(emb)) in conv1's epilogue; the VAE's have no time embedding
   Lin temb;
   bool has_sc = false;
   Lin sc;
@@ -132,6 +133,14 @@ struct MotionW {
 struct CamResW {
   Conv3 block1;
   Lin block2;
+};
+struct VaeAttnW {   // AutoencoderKL mid-block attention: one head of C = 512 channels, biased q / k / v
+  Norm gn;
+  Mat wqk;          // [2C][C]: to_q rows then to_k rows
+  __half* bqk = nullptr;
+  Mat wv;           // [C][C] (the "A" operand of the V^T GEMM)
+  __half* bv = nullptr;
+  Lin out;
 };
 
 // ------------------------------------------------------------------------------------------ workspace arena
@@ -249,6 +258,17 @@ struct hv_model {
   std::vector<CamResW> cam_res;
   std::vector<MotionW> cam_att;  // reuse MotionW: attn[0] + ff (no gn / proj)
   Lin cam_zero;
+  // ---- AutoencoderKL: encoder.* / decoder.* (the down / up blocks and the mid block's two resnets are Stages without attention)
+  struct VaeHalf {
+    Conv3 conv_in;
+    std::vector<Stage> blocks;
+    Stage mid;
+    VaeAttnW attn;
+    Norm norm_out;
+    Conv3 conv_out;
+  };
+  VaeHalf enc, dec;
+  Lin quant, post_quant;   // post_quant_conv zero-padded to [64][64]: its output is conv_in's 64-channel padded input
 
   ~hv_model() {
     for (void* p : owned) cudaFree(p);
@@ -357,14 +377,16 @@ struct hv_model {
     return l;
   }
 
-  ResnetW resnet(const std::string& pfx, int cin, int cout, int temb) {
+  // temb == 0: a resnet without time embedding (no time_emb_proj)
+  ResnetW resnet(const std::string& pfx, int cin, int cout, int temb, float eps = 1e-5f) {
     ResnetW r;
     r.cin = cin;
     r.cout = cout;
-    r.n1 = norm(pfx + ".norm1", cin, 1e-5f);
+    r.n1 = norm(pfx + ".norm1", cin, eps);
     r.c1 = conv3(pfx + ".conv1", cout, cin);
-    r.temb = lin(pfx + ".time_emb_proj", cout, temb);
-    r.n2 = norm(pfx + ".norm2", cout, 1e-5f);
+    r.has_temb = temb > 0;
+    if (r.has_temb) r.temb = lin(pfx + ".time_emb_proj", cout, temb);
+    r.n2 = norm(pfx + ".norm2", cout, eps);
     r.c2 = conv3(pfx + ".conv2", cout, cout);
     r.has_sc = cin != cout;
     if (r.has_sc) r.sc = lin(pfx + ".conv_shortcut", cout, cin);
@@ -541,6 +563,86 @@ struct hv_model {
     cam_zero = lin("zero_conv_layers.0", C, C, false);
   }
 
+  // ---- AutoencoderKL (diffusers 0.24 key names; SD layout: 4 levels, 2 resnets per encoder level, 3 per decoder level)
+  // [n_pad][k_pad] zero-padded copy of an [n][k] linear / 1x1 conv weight, bias zero-padded to n_pad
+  Lin padded_linear(const std::string& pfx, int n, int k, int n_pad, int k_pad) {
+    const Raw& w = get(pfx + ".weight");
+    if (w.numel() != static_cast<int64_t>(n) * k) fail(HV_ERR_INVALID, "weight '%s.weight' has %lld elements, expected %d x %d", pfx.c_str(), (long long)w.numel(), n, k);
+    Lin l;
+    l.w = Mat{dmalloc(static_cast<int64_t>(n_pad) * k_pad), n_pad, k_pad};
+    ck(cudaMemsetAsync(l.w.p, 0, static_cast<size_t>(n_pad) * k_pad * 2, st), "memset");
+    ck(cudaMemcpy2DAsync(l.w.p, static_cast<size_t>(k_pad) * 2, w.p, static_cast<size_t>(k) * 2, static_cast<size_t>(k) * 2, n, cudaMemcpyDeviceToDevice, st),
+       "padded weight copy");
+    l.bias = vec(pfx + ".bias", n, n_pad);
+    return l;
+  }
+  VaeAttnW vae_attn(const std::string& pfx, int C) {
+    if (C != 512) fail(HV_ERR_INVALID, "'%s': the mid-block attention is implemented for 512 channels (one head of d = 512), got %d", pfx.c_str(), C);
+    VaeAttnW a;
+    a.gn = norm(pfx + ".group_norm", C, 1e-6f);
+    a.wqk = Mat{dmalloc(2LL * C * C), 2LL * C, C};
+    a.bqk = dmalloc(2LL * C);
+    const char* qk[2] = {".to_q", ".to_k"};
+    for (int i = 0; i < 2; ++i) {
+      ck(cudaMemcpyAsync(a.wqk.p + static_cast<int64_t>(i) * C * C, mat(pfx + qk[i] + ".weight", C, C).p, static_cast<size_t>(C) * C * 2, cudaMemcpyDeviceToDevice, st),
+         "q/k concat");
+      ck(cudaMemcpyAsync(a.bqk + static_cast<int64_t>(i) * C, vec(pfx + qk[i] + ".bias", C), static_cast<size_t>(C) * 2, cudaMemcpyDeviceToDevice, st), "q/k bias concat");
+    }
+    a.wv = mat(pfx + ".to_v.weight", C, C);
+    a.bv = vec(pfx + ".to_v.bias", C);
+    a.out = lin(pfx + ".to_out.0", C, C);
+    return a;
+  }
+  // a stage of n resnets (the first one ins -> C, the others C -> C), GroupNorm eps 1e-6, no time embedding
+  Stage vae_stage(const std::string& name, int ins, int C, int n) {
+    Stage s;
+    s.name = name;
+    for (int j = 0; j < n; ++j) s.res.push_back(resnet(name + ".resnets." + std::to_string(j), j == 0 ? ins : C, C, 0, 1e-6f));
+    return s;
+  }
+  void build_vae() {
+    const int* ch = cfg.block_out_channels;
+    const int zc = cfg.vae_latent_channels;
+    if (zc <= 0 || zc > 64 || (2 * zc) % 8) fail(HV_ERR_INVALID, "vae_latent_channels = %d: 2 * latent channels must be a multiple of 8 and <= 128", zc);
+    if (cfg.in_channels <= 0 || cfg.in_channels > 64 || cfg.out_channels <= 0 || cfg.out_channels > 64)
+      fail(HV_ERR_INVALID, "AutoencoderKL image channels (%d in, %d out) must be 1..64", cfg.in_channels, cfg.out_channels);
+    // encoder: conv_in, 4 x DownEncoderBlock2D (the first three end in Downsample2D: pad (0, 1, 0, 1) + stride-2 conv), mid block,
+    // conv_norm_out + SiLU, conv_out -> 2 * latent channels (mean | logvar)
+    enc.conv_in = conv3("encoder.conv_in", ch[0], cfg.in_channels);
+    enc.blocks.clear();
+    int prev = ch[0];
+    for (int i = 0; i < 4; ++i) {
+      Stage s = vae_stage("encoder.down_blocks." + std::to_string(i), prev, ch[i], 2);
+      s.has_sampler = i < 3;
+      if (s.has_sampler) s.sampler = conv3(s.name + ".downsamplers.0.conv", ch[i], ch[i]);
+      enc.blocks.push_back(std::move(s));
+      prev = ch[i];
+    }
+    enc.mid = vae_stage("encoder.mid_block", ch[3], ch[3], 2);
+    enc.attn = vae_attn("encoder.mid_block.attentions.0", ch[3]);
+    enc.norm_out = norm("encoder.conv_norm_out", ch[3], 1e-6f);
+    enc.conv_out = conv3("encoder.conv_out", 2 * zc, ch[3]);
+    quant = lin("quant_conv", 2 * zc, 2 * zc);
+    // decoder: post_quant_conv, conv_in, mid block, 4 x UpDecoderBlock2D over (ch3, ch2, ch1, ch0) (the first three end in nearest 2x +
+    // 3x3 conv), conv_norm_out + SiLU, conv_out
+    post_quant = padded_linear("post_quant_conv", zc, zc, 64, 64);
+    dec.conv_in = conv3("decoder.conv_in", ch[3], zc);
+    dec.mid = vae_stage("decoder.mid_block", ch[3], ch[3], 2);
+    dec.attn = vae_attn("decoder.mid_block.attentions.0", ch[3]);
+    dec.blocks.clear();
+    prev = ch[3];
+    for (int i = 0; i < 4; ++i) {
+      const int c = ch[3 - i];
+      Stage s = vae_stage("decoder.up_blocks." + std::to_string(i), prev, c, 3);
+      s.has_sampler = i < 3;
+      if (s.has_sampler) s.sampler = upconv(s.name + ".upsamplers.0.conv", c, c);
+      dec.blocks.push_back(std::move(s));
+      prev = c;
+    }
+    dec.norm_out = norm("decoder.conv_norm_out", ch[0], 1e-6f);
+    dec.conv_out = conv3("decoder.conv_out", cfg.out_channels, ch[0]);
+  }
+
   // ================================================================== op wrappers (no-ops while measuring)
   Tens alloc_act(int NF, int H, int W, int C) {
     Tens a;
@@ -590,7 +692,9 @@ struct hv_model {
     gemm(x.p, x.C, nullptr, 0, 0, l.w, out.p, N, x.rows(), &ep);
     return out;
   }
-  Tens op_conv3(const Tens& x, const Conv3& c, int stride, const __half* rowvec, int64_t rows_per_group, int act, const Tens* residual) {
+  // pad_end: stride 2 with padding (0, 1, 0, 1) (AutoencoderKL's Downsample2D) instead of 1 on every side
+  Tens op_conv3(const Tens& x, const Conv3& c, int stride, const __half* rowvec, int64_t rows_per_group, int act, const Tens* residual,
+                bool pad_end = false) {
     if (x.C != c.cin_pad) fail(HV_ERR_INVALID, "conv3x3: input has %d channels, weight packed for %d", x.C, c.cin_pad);
     const int Ho = stride == 1 ? x.H : x.H / 2, Wo = stride == 1 ? x.W : x.W / 2;
     Tens out = alloc_act(x.NF, Ho, Wo, c.cout_pad);
@@ -601,9 +705,19 @@ struct hv_model {
     ep.rows_per_group = static_cast<int32_t>(rows_per_group);
     ep.act = act;
     if (residual) { ep.residual = residual->p; ep.ldr = residual->C; }
-    launch(1, {CAT_CONV, stride == 1 ? "conv3" : "conv3_s2", 2.0 * out.rows() * c.cout * 9.0 * c.cin, out.rows(), c.cout_pad, 9LL * c.cin_pad},
-           [&] { ckop(op_conv3x3(x.p, c.w.p, out.p, c.cout_pad, x.NF, x.H, x.W, c.cin_pad, c.cout_pad, stride, &ep, st), "conv3x3"); });
+    launch(1, {CAT_CONV, stride == 1 ? "conv3" : (pad_end ? "conv3_s2_end" : "conv3_s2"), 2.0 * out.rows() * c.cout * 9.0 * c.cin, out.rows(), c.cout_pad,
+               9LL * c.cin_pad},
+           [&] { ckop(op_conv3x3(x.p, c.w.p, out.p, c.cout_pad, x.NF, x.H, x.W, c.cin_pad, c.cout_pad, stride, &ep, st, pad_end), "conv3x3"); });
     return out;
+  }
+  // Upsample3D / Upsample2D: nearest 2x + 3x3 conv as four 2x2 convs of the source -- the 4x tensor is never materialised
+  Tens op_upconv(const Tens& h, const Conv3& c) {
+    Tens big = alloc_act(h.NF, 2 * h.H, 2 * h.W, c.cout);
+    hv_epilogue ep{};
+    ep.bias = c.bias;
+    launch(1, {CAT_CONV, "upconv2x2", 2.0 * big.rows() * c.cout * 4.0 * c.cin, big.rows(), c.cout, 4LL * c.cin},
+           [&] { ckop(op_upconv2x2(h.p, c.w.p, big.p, c.cout, h.NF, h.H, h.W, c.cin, c.cout, &ep, st), "upsampler conv"); });
+    return big;
   }
   __half* op_small_linear(const __half* x, const Lin& l, int M, int act_in) {
     __half* out = alloc_h(static_cast<int64_t>(M) * l.w.rows);
@@ -623,7 +737,7 @@ struct hv_model {
       out = alloc_act(x.NF, x.H, x.W, r.cout);
     }
     Scope s(ar);
-    __half* tproj = op_small_linear(emb, r.temb, B, HV_ACT_SILU);  // time_emb_proj(silu(emb)) : [B][cout]
+    __half* tproj = r.has_temb ? op_small_linear(emb, r.temb, B, HV_ACT_SILU) : nullptr;  // time_emb_proj(silu(emb)) : [B][cout]
     Tens h = op_gn(x, x2, r.n1, true);
     Tens h1 = op_conv3(h, r.c1, 1, tproj, static_cast<int64_t>(F) * x.H * x.W, HV_ACT_NONE, nullptr);
     Tens h2 = op_gn(h1, nullptr, r.n2, true);
@@ -853,14 +967,7 @@ struct hv_model {
         layer(s, j, &skip);
       }
       if (s.has_sampler) {
-        // Upsample3D (resnet.py:68-71): nearest 2x + 3x3 conv as four 2x2 convs of the source -- the 4x tensor is never materialised
-        const Conv3& c = s.sampler;
-        Tens big = alloc_act(h.NF, 2 * h.H, 2 * h.W, c.cout);
-        hv_epilogue ep{};
-        ep.bias = c.bias;
-        launch(1, {CAT_CONV, "upconv2x2", 2.0 * big.rows() * c.cout * 4.0 * c.cin, big.rows(), c.cout, 4LL * c.cin},
-               [&] { ckop(op_upconv2x2(h.p, c.w.p, big.p, c.cout, h.NF, h.H, h.W, c.cin, c.cout, &ep, st), "upsampler conv"); });
-        h = big;
+        h = op_upconv(h, s.sampler);   // Upsample3D (resnet.py:68-71)
         tap(s.name + ".upsamplers.0", h);
       }
     }
@@ -940,6 +1047,80 @@ struct hv_model {
     Tens z = op_linear(x, cam_zero, nullptr);
     launch(1, {}, [&] { ck(launch_nhwc_to_ncfhw(z.p, z.C, outp, NF, C, 1, z.H, z.W, st), "camera output layout"); });
   }
+
+  // ================================================================== AutoencoderKL
+  // diffusers Attention of the VAE mid block: GroupNorm -> q, k, v (+bias) -> one head of d = 512 -> to_out (+bias) + residual.  Q and
+  // K come from one GEMM, V^T (frames side by side) from the swapped GEMM with to_v's bias as its row bias.
+  Tens vae_attn_fwd(const VaeAttnW& w, const Tens& x) {
+    Tens out = alloc_act(x.NF, x.H, x.W, x.C);
+    Scope s(ar);
+    const int C = x.C, L = x.H * x.W;
+    const int64_t tokens = x.rows();
+    Tens hn = op_gn(x, nullptr, w.gn, false);
+    __half* qk = alloc_h(tokens * 2 * C);
+    hv_epilogue eqk{};
+    eqk.bias = w.bqk;
+    gemm(hn.p, C, nullptr, 0, 0, w.wqk, qk, 2 * C, tokens, &eqk);
+    const int64_t Lp = rup(L, 8), ldvt = static_cast<int64_t>(x.NF) * Lp;
+    __half* vt = alloc_h(C * ldvt);
+    launch(1, {CAT_GEMM, "gemm_vt", 2.0 * tokens * C * C, C, tokens, C},
+           [&] { ckop(op_gemm_batched_b(w.wv.p, C, hn.p, C, vt, ldvt, C, x.NF, L, Lp, C, w.bv, st), "V^T gemm"); });
+    Tens o = alloc_act(x.NF, x.H, x.W, C);
+    launch(1, {CAT_ATTN, "attn_d512", 4.0 * x.NF * static_cast<double>(L) * L * C, x.NF, L, C}, [&] {
+      cudaError_t e = launch_attention_d512(qk, 2 * C, qk + C, 2 * C, vt, ldvt, Lp, o.p, C, x.NF, L, st);
+      if (e != cudaSuccess) fail(HV_ERR_CUDA, "attention d512: %s %s", cudaGetErrorString(e), tma_last_error());
+    });
+    hv_epilogue ep{};
+    ep.bias = w.out.bias;
+    ep.residual = x.p;
+    ep.ldr = x.C;
+    gemm(o.p, C, nullptr, 0, 0, w.out.w, out.p, C, tokens, &ep);
+    return out;
+  }
+  // UNetMidBlock2D: resnet, attention, resnet
+  Tens vae_mid_fwd(const VaeHalf& v, Tens h) {
+    h = resnet_fwd(v.mid.res[0], h, nullptr, nullptr, h.NF, 1);
+    h = vae_attn_fwd(v.attn, h);
+    return resnet_fwd(v.mid.res[1], h, nullptr, nullptr, h.NF, 1);
+  }
+  // Every operator works per frame (per-frame GroupNorm statistics, per-frame attention), so frame i of a call does not depend on the
+  // other frames of the call.
+  void vae_encode(const __half* x, __half* moments, int N, int H, int W) {
+    if (N <= 0 || H <= 0 || W <= 0 || (H % 8) || (W % 8)) fail(HV_ERR_INVALID, "AutoencoderKL.encode: N = %d images of %dx%d: N must be > 0 and H, W positive multiples of 8", N, H, W);
+    Tens x0 = alloc_act(N, H, W, enc.conv_in.cin_pad);   // the image channels zero-padded to one 64-wide k-block
+    launch(2, {}, [&] {
+      ck(cudaMemsetAsync(x0.p, 0, static_cast<size_t>(x0.numel()) * 2, st), "memset");
+      ck(launch_ncfhw_to_nhwc(x, x0.p, N, cfg.in_channels, 1, H, W, 0, st, x0.C), "image layout");
+    });
+    Tens h = op_conv3(x0, enc.conv_in, 1, nullptr, 1, HV_ACT_NONE, nullptr);
+    for (const Stage& s : enc.blocks) {
+      for (const ResnetW& r : s.res) h = resnet_fwd(r, h, nullptr, nullptr, N, 1);
+      if (s.has_sampler) h = op_conv3(h, s.sampler, 2, nullptr, 1, HV_ACT_NONE, nullptr, true);   // Downsample2D: pad (0, 1, 0, 1), stride 2
+    }
+    h = vae_mid_fwd(enc, h);
+    Tens hn = op_gn(h, nullptr, enc.norm_out, true);
+    Tens y = op_conv3(hn, enc.conv_out, 1, nullptr, 1, HV_ACT_NONE, nullptr);
+    Tens m = op_linear(y, quant, nullptr);   // quant_conv (1x1)
+    launch(1, {}, [&] { ck(launch_nhwc_to_ncfhw(m.p, m.C, moments, N, m.C, 1, m.H, m.W, st), "moments layout"); });
+  }
+  void vae_decode(const __half* z, __half* outp, int N, int H, int W) {
+    if (N <= 0 || H <= 0 || W <= 0) fail(HV_ERR_INVALID, "AutoencoderKL.decode: N = %d latents of %dx%d must all be positive", N, H, W);
+    Tens z0 = alloc_act(N, H, W, static_cast<int>(post_quant.w.cols));   // latent channels zero-padded to 64
+    launch(2, {}, [&] {
+      ck(cudaMemsetAsync(z0.p, 0, static_cast<size_t>(z0.numel()) * 2, st), "memset");
+      ck(launch_ncfhw_to_nhwc(z, z0.p, N, cfg.vae_latent_channels, 1, H, W, 0, st, z0.C), "latent layout");
+    });
+    Tens p = op_linear(z0, post_quant, nullptr);   // post_quant_conv (1x1); its padded channels stay zero for conv_in
+    Tens h = op_conv3(p, dec.conv_in, 1, nullptr, 1, HV_ACT_NONE, nullptr);
+    h = vae_mid_fwd(dec, h);
+    for (const Stage& s : dec.blocks) {
+      for (const ResnetW& r : s.res) h = resnet_fwd(r, h, nullptr, nullptr, N, 1);
+      if (s.has_sampler) h = op_upconv(h, s.sampler);
+    }
+    Tens hn = op_gn(h, nullptr, dec.norm_out, true);
+    Tens y = op_conv3(hn, dec.conv_out, 1, nullptr, 1, HV_ACT_NONE, nullptr);
+    launch(1, {}, [&] { ck(launch_nhwc_to_ncfhw(y.p, y.C, outp, N, cfg.out_channels, 1, y.H, y.W, st), "image output layout"); });
+  }
 };
 
 // ------------------------------------------------------------------------------------------ C ABI
@@ -982,6 +1163,12 @@ static size_t measure(hv_model* h, int B, int F, int H, int W, uint32_t flags = 
     h->unet_forward(&dummy, 0, &dummy, h->cfg.kind == HV_KIND_UNET3D ? &dummy : nullptr, &dummy, B, F, H, W, flags);
   } else if (h->cfg.kind == HV_KIND_POSE_GUIDER) {
     h->pose_guider_forward(nullptr, nullptr, B, F, H, W);
+  } else if (h->cfg.kind == HV_KIND_VAE) {   // (H, W) = latent size: the workspace covers decoding B latents and encoding B images of 8H x 8W
+    h->vae_decode(nullptr, nullptr, B, H, W);
+    const size_t dec_peak = h->ar.peak;
+    h->begin(nullptr, 0, true, nullptr);
+    h->vae_encode(nullptr, nullptr, B, 8 * H, 8 * W);
+    return std::max(dec_peak, h->ar.peak) + 4096;
   } else {
     h->camera_forward(nullptr, nullptr, B, F, H, W);
   }
@@ -1011,7 +1198,7 @@ int hv_create(const hv_config* cfg, hv_handle* out) {
     m = new hv_model();
     m->cfg = *cfg;
     m->sms = sms;
-    if (cfg->kind < 0 || cfg->kind > 3) fail(HV_ERR_INVALID, "unknown kind %d", cfg->kind);
+    if (cfg->kind < 0 || cfg->kind > HV_KIND_VAE) fail(HV_ERR_INVALID, "unknown kind %d", cfg->kind);
     if (cfg->kind == HV_KIND_UNET2D_REF && cfg->use_motion_module) fail(HV_ERR_INVALID, "the reference (writer) UNet has no motion modules");
     *out = m;
     return HV_OK;
@@ -1103,6 +1290,7 @@ int hv_finalize(hv_handle h, hv_stream_t stream) {
     h->st = static_cast<cudaStream_t>(stream);
     if (h->cfg.kind == HV_KIND_UNET3D || h->cfg.kind == HV_KIND_UNET2D_REF) h->build_unet();
     else if (h->cfg.kind == HV_KIND_POSE_GUIDER) h->build_pose_guider();
+    else if (h->cfg.kind == HV_KIND_VAE) h->build_vae();
     else h->build_camera();
     h->finalized = true;
   });
@@ -1244,6 +1432,26 @@ int hv_camera_encoder_forward_rays(hv_handle h, const float* intrinsics, const f
   return guard(h, [&] {
     run_forward(h, HV_KIND_CAMERA_ENCODER, "CameraPoseEncoder", B, F, H, W, HV_FLAG_CFG, workspace, ws_bytes, stream,
                 [&] { h->camera_forward(nullptr, static_cast<__half*>(out), B, F, H, W, intrinsics, c2w); });
+  });
+}
+
+int hv_vae_decode(hv_handle h, const void* z, void* out, int32_t N, int32_t height, int32_t width, void* workspace, size_t ws_bytes,
+                  hv_stream_t stream) {
+  if (!h || !z || !out) return HV_ERR_INVALID;
+  return guard(h, [&] {
+    run_forward(h, HV_KIND_VAE, "AutoencoderKL", N, 1, height, width, 0, workspace, ws_bytes, stream,
+                [&] { h->vae_decode(static_cast<const __half*>(z), static_cast<__half*>(out), N, height, width); });
+  });
+}
+
+int hv_vae_encode(hv_handle h, const void* x, void* moments, int32_t N, int32_t H, int32_t W, void* workspace, size_t ws_bytes,
+                  hv_stream_t stream) {
+  if (!h || !x || !moments) return HV_ERR_INVALID;
+  return guard(h, [&] {
+    if (N <= 0 || H <= 0 || W <= 0 || (H % 8) || (W % 8))
+      fail(HV_ERR_INVALID, "AutoencoderKL.encode: N = %d images of %dx%d: N must be > 0 and H, W positive multiples of 8", N, H, W);
+    run_forward(h, HV_KIND_VAE, "AutoencoderKL", N, 1, H / 8, W / 8, 0, workspace, ws_bytes, stream,
+                [&] { h->vae_encode(static_cast<const __half*>(x), static_cast<__half*>(moments), N, H, W); });
   });
 }
 

@@ -161,17 +161,17 @@ static void set_conv_tiles(GemmProblem& p, int64_t NF, int64_t H, int64_t W) {
 }
 
 int op_conv3x3(const __half* X, const __half* Wp, __half* out, int64_t ldc, int64_t NF, int64_t H, int64_t W, int64_t Cin,
-               int64_t Cout, int stride, const hv_epilogue* ep, cudaStream_t stream) {
+               int64_t Cout, int stride, const hv_epilogue* ep, cudaStream_t stream, bool pad_end) {
   const int sms = device_sms();
   if (!sms) return HV_ERR_CUDA;
-  if ((Cin % 64) || (Cout % 8) || (ldc % 8) || (stride != 1 && stride != 2) || NF <= 0 || H <= 0 || W <= 0) {
+  if ((Cin % 64) || (Cout % 8) || (ldc % 8) || (stride != 1 && stride != 2) || (pad_end && stride != 2) || NF <= 0 || H <= 0 || W <= 0) {
     set_error("hv_op_conv3x3: bad shape NF=%lld H=%lld W=%lld Cin=%lld Cout=%lld stride=%d", (long long)NF, (long long)H, (long long)W,
               (long long)Cin, (long long)Cout, stride);
     return HV_ERR_INVALID;
   }
   const int64_t Ho = stride == 1 ? H : H / 2, Wo = stride == 1 ? W : W / 2;
   GemmProblem p;
-  p.a_mode = stride == 1 ? A_CONV3X3 : A_CONV3X3_S2;
+  p.a_mode = stride == 1 ? A_CONV3X3 : (pad_end ? A_CONV3X3_S2_END : A_CONV3X3_S2);
   p.N = static_cast<int>(Cout);
   p.cin_blocks = static_cast<int>(Cin / 64);
   p.cin = static_cast<int>(Cin);

@@ -60,6 +60,16 @@ bool make_map_3d(CUtensorMap* m, const void* ptr, int64_t batch, int64_t rows, i
   return encode(m, ptr, 3, dims, strides, box);
 }
 
+bool make_map_col_batches(CUtensorMap* m, const void* ptr, int64_t batch, int64_t rows, int64_t cols, int64_t ld, int64_t batch_stride,
+                          int box_rows) {
+  // the batch axis is the middle one so that the strides grow outwards (batch_stride <= ld); a box of one item has the same
+  // shared-memory layout as (64, box_rows)
+  cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)batch, (cuuint64_t)rows};
+  cuuint64_t strides[2] = {(cuuint64_t)batch_stride * 2, (cuuint64_t)ld * 2};
+  cuuint32_t box[3] = {64, 1, (cuuint32_t)box_rows};
+  return encode(m, ptr, 3, dims, strides, box);
+}
+
 bool make_map_frames(CUtensorMap* m, const void* ptr, int64_t frames, int64_t pixels, int64_t cols, int64_t ld, int box_cols, int box_frames) {
   cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)pixels, (cuuint64_t)frames};
   cuuint64_t strides[2] = {(cuuint64_t)ld * 2, (cuuint64_t)pixels * ld * 2};

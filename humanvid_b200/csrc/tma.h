@@ -25,6 +25,12 @@ bool make_map_nhwc_s2(CUtensorMap* m, const void* ptr, int64_t N, int64_t H, int
 // even when the next batch item follows in memory.
 bool make_map_3d(CUtensorMap* m, const void* ptr, int64_t batch, int64_t rows, int64_t cols, int64_t ld, int box_rows);
 
+// fp16 [rows][ld] matrix whose batch item n occupies columns [n * batch_stride, n * batch_stride + cols) (batch_stride % 8 == 0)
+// -> 3-D map (cols, batch, rows), box (64, 1, box_rows), coordinates (col, item, row); columns beyond `cols` read as zero even
+// when the next item follows (V^T with the frames side by side).
+bool make_map_col_batches(CUtensorMap* m, const void* ptr, int64_t batch, int64_t rows, int64_t cols, int64_t ld, int64_t batch_stride,
+                          int box_rows);
+
 // Token matrix [frames][pixels][ld] (cols valid) viewed along the frame axis: 3-D map (cols, pixels, frames), unswizzled box
 // (box_cols, 1, box_frames) = the box_frames rows of ONE pixel, box_cols channels wide (temporal attention operands).
 bool make_map_frames(CUtensorMap* m, const void* ptr, int64_t frames, int64_t pixels, int64_t cols, int64_t ld, int box_cols, int box_frames);

@@ -9,6 +9,8 @@
   * ``CameraPoseEncoder.forward``     <->  src/cameractrl/pose_adaptor.py:232-248
   * ``UNet2DConditionModel.forward``  <->  src/models/unet_2d_condition.py:872-1308 (the reference / "writer" UNet, whose
     LayerNorm-1 outputs become the denoising UNet's K/V banks)
+  * ``AutoencoderKL.encode / decode``  <->  diffusers 0.24 ``AutoencoderKL`` in the SD layout (sd-vae-ft-mse), what the pipelines
+    call for the reference latents and the output frames
 
 The ``nn.Module`` tree below only *holds parameters* under the reference's names (torch is plumbing: device memory,
 ``load_state_dict``, ``.to()``); none of its sub-modules' ``forward`` is ever executed.  All arithmetic happens in
@@ -347,6 +349,7 @@ class HvConfig(C.Structure):
         ("cam_nums_rb", C.c_int32),
         ("cam_heads", C.c_int32),
         ("cam_max_len", C.c_int32),
+        ("vae_latent_channels", C.c_int32),
     ]
 
 
@@ -982,3 +985,273 @@ class ReferenceAttentionControl:
         else:
             for m, _ in self.unet.writer_blocks():
                 m.bank.clear()
+
+
+# --------------------------------------------------------------------------------------------- AutoencoderKL
+class _VaeResnet(_Shell):
+    """diffusers ResnetBlock2D with temb_channels=None (no time_emb_proj), GroupNorm eps 1e-6."""
+
+    def __init__(self, cin, cout, groups):
+        super().__init__()
+        self.norm1 = nn.GroupNorm(groups, cin, eps=1e-6)
+        self.conv1 = _conv(cin, cout, 3, padding=1)
+        self.norm2 = nn.GroupNorm(groups, cout, eps=1e-6)
+        self.conv2 = _conv(cout, cout, 3, padding=1)
+        if cin != cout:
+            self.conv_shortcut = _conv(cin, cout, 1)
+
+
+class _VaeAttention(_Shell):
+    """diffusers Attention of the VAE mid block: group_norm, to_q / to_k / to_v WITH bias, one head, to_out.0."""
+
+    def __init__(self, ch, groups):
+        super().__init__()
+        self.group_norm = nn.GroupNorm(groups, ch, eps=1e-6)
+        self.to_q = nn.Linear(ch, ch)
+        self.to_k = nn.Linear(ch, ch)
+        self.to_v = nn.Linear(ch, ch)
+        self.to_out = nn.ModuleList([nn.Linear(ch, ch), nn.Dropout(0.0)])
+
+
+class _VaeDownsample(_Shell):
+    """Downsample2D(use_conv=True, padding=0): F.pad(x, (0, 1, 0, 1)) then a 3x3 stride-2 conv."""
+
+    def __init__(self, ch):
+        super().__init__()
+        self.conv = _conv(ch, ch, 3, stride=2, padding=0)
+
+
+class _VaeBlock(_Shell):
+    def __init__(self, cin, cout, n, groups, sampler=None):
+        super().__init__()
+        self.resnets = nn.ModuleList([_VaeResnet(cin if j == 0 else cout, cout, groups) for j in range(n)])
+        if sampler == "down":
+            self.downsamplers = nn.ModuleList([_VaeDownsample(cout)])
+        elif sampler == "up":
+            self.upsamplers = nn.ModuleList([_Sampler(cout, 1)])
+
+
+class _VaeMid(_Shell):
+    def __init__(self, ch, groups):
+        super().__init__()
+        self.attentions = nn.ModuleList([_VaeAttention(ch, groups)])
+        self.resnets = nn.ModuleList([_VaeResnet(ch, ch, groups), _VaeResnet(ch, ch, groups)])
+
+
+class _VaeEncoder(_Shell):
+    def __init__(self, cin, ch, latent, groups, layers):
+        super().__init__()
+        self.conv_in = _conv(cin, ch[0], 3, padding=1)
+        self.down_blocks = nn.ModuleList([_VaeBlock(ch[max(i - 1, 0)], c, layers, groups, "down" if i < len(ch) - 1 else None) for i, c in enumerate(ch)])
+        self.mid_block = _VaeMid(ch[-1], groups)
+        self.conv_norm_out = nn.GroupNorm(groups, ch[-1], eps=1e-6)
+        self.conv_out = _conv(ch[-1], 2 * latent, 3, padding=1)
+
+
+class _VaeDecoder(_Shell):
+    def __init__(self, cout, ch, latent, groups, layers):
+        super().__init__()
+        rev = list(ch)[::-1]
+        self.conv_in = _conv(latent, rev[0], 3, padding=1)
+        self.mid_block = _VaeMid(rev[0], groups)
+        self.up_blocks = nn.ModuleList([_VaeBlock(rev[max(i - 1, 0)], c, layers + 1, groups, "up" if i < len(rev) - 1 else None) for i, c in enumerate(rev)])
+        self.conv_norm_out = nn.GroupNorm(groups, ch[0], eps=1e-6)
+        self.conv_out = _conv(ch[0], cout, 3, padding=1)
+
+
+class DiagonalGaussianDistribution:
+    """The posterior ``encode`` returns: ``moments`` = [mean | logvar] over the channel axis (diffusers' class of the same name; what the
+    pipelines read is ``mean``)."""
+
+    def __init__(self, parameters: torch.Tensor):
+        self.parameters = parameters
+        self.mean, logvar = torch.chunk(parameters, 2, dim=1)
+        self.logvar = torch.clamp(logvar, -30.0, 20.0)
+
+    @property
+    def std(self):
+        return torch.exp(0.5 * self.logvar)
+
+    @property
+    def var(self):
+        return torch.exp(self.logvar)
+
+    def mode(self):
+        return self.mean
+
+
+@dataclass
+class AutoencoderKLOutput:
+    latent_dist: DiagonalGaussianDistribution
+
+
+@dataclass
+class DecoderOutput:
+    sample: torch.Tensor
+
+
+# attention parameter names of diffusers < 0.14 checkpoints -> the current ones (diffusers converts them the same way on load)
+_VAE_LEGACY_ATTN = {"query": "to_q", "key": "to_k", "value": "to_v", "proj_attn": "to_out.0"}
+
+
+def _convert_legacy_vae_keys(state):
+    out = {}
+    for k, v in state.items():
+        parts = k.split(".")
+        if len(parts) == 6 and parts[0] in ("encoder", "decoder") and parts[1:4] == ["mid_block", "attentions", "0"] and parts[4] in _VAE_LEGACY_ATTN:
+            k = ".".join(parts[:4] + [_VAE_LEGACY_ATTN[parts[4]], parts[5]])
+            if parts[5] == "weight" and v.dim() == 4:   # stored as a 1x1 conv
+                v = v[:, :, 0, 0]
+        out[k] = v
+    return out
+
+
+class AutoencoderKL(_NativeNet):
+    """Drop-in for diffusers' ``AutoencoderKL`` (0.24) in the SD layout that configs/prompts/stage2.yaml points at (sd-vae-ft-mse):
+    same constructor keywords, ``config``, ``state_dict`` keys, ``from_pretrained``, ``encode(x).latent_dist.mean`` and
+    ``decode(z).sample``.  Both run on libhv_b200 (``hv_vae_encode`` / ``hv_vae_decode``); every frame of a call is computed independently of
+    the others.  Inference only: no tiling / slicing, no ``latent_dist.sample()``.
+    """
+
+    _kind = 4
+
+    def __init__(
+        self,
+        in_channels: int = 3,
+        out_channels: int = 3,
+        down_block_types: Tuple[str, ...] = ("DownEncoderBlock2D",) * 4,
+        up_block_types: Tuple[str, ...] = ("UpDecoderBlock2D",) * 4,
+        block_out_channels: Tuple[int, ...] = (128, 256, 512, 512),
+        layers_per_block: int = 2,
+        act_fn: str = "silu",
+        latent_channels: int = 4,
+        norm_num_groups: int = 32,
+        sample_size: int = 512,
+        scaling_factor: float = 0.18215,
+        force_upcast: bool = True,
+        **unused,
+    ):
+        super().__init__()
+        unsupported = []
+        if tuple(down_block_types) != ("DownEncoderBlock2D",) * 4 or tuple(up_block_types) != ("UpDecoderBlock2D",) * 4:
+            unsupported.append(f"block types {tuple(down_block_types)} / {tuple(up_block_types)} (4 x DownEncoderBlock2D / UpDecoderBlock2D)")
+        if tuple(block_out_channels) != (128, 256, 512, 512):
+            unsupported.append(f"block_out_channels {tuple(block_out_channels)} (128, 256, 512, 512)")
+        if layers_per_block != 2:
+            unsupported.append(f"layers_per_block {layers_per_block} (2)")
+        if act_fn not in ("silu", "swish"):
+            unsupported.append(f"act_fn {act_fn!r} (silu)")
+        if norm_num_groups != 32:
+            unsupported.append(f"norm_num_groups {norm_num_groups} (32)")
+        if latent_channels != 4:
+            unsupported.append(f"latent_channels {latent_channels} (4)")
+        if not (1 <= in_channels <= 64 and 1 <= out_channels <= 64):
+            unsupported.append(f"in_channels / out_channels {in_channels} / {out_channels} (1..64)")
+        if unsupported:
+            raise NotImplementedError("humanvid_b200.AutoencoderKL implements the SD VAE layout only; unsupported: " + "; ".join(unsupported))
+        self.config = SimpleNamespace(in_channels=in_channels, out_channels=out_channels, down_block_types=tuple(down_block_types),
+                                      up_block_types=tuple(up_block_types), block_out_channels=tuple(block_out_channels),
+                                      layers_per_block=layers_per_block, act_fn=act_fn, latent_channels=latent_channels,
+                                      norm_num_groups=norm_num_groups, sample_size=sample_size, scaling_factor=scaling_factor,
+                                      force_upcast=force_upcast)
+        ch = list(block_out_channels)
+        self.encoder = _VaeEncoder(in_channels, ch, latent_channels, norm_num_groups, layers_per_block)
+        self.decoder = _VaeDecoder(out_channels, ch, latent_channels, norm_num_groups, layers_per_block)
+        self.quant_conv = _conv(2 * latent_channels, 2 * latent_channels, 1)
+        self.post_quant_conv = _conv(latent_channels, latent_channels, 1)
+
+    def _hv_config(self):
+        c = self.config
+        cfg = HvConfig()
+        cfg.kind = 4
+        cfg.in_channels, cfg.out_channels = c.in_channels, c.out_channels
+        cfg.block_out_channels = (C.c_int32 * 4)(*c.block_out_channels)
+        cfg.norm_groups = c.norm_num_groups
+        cfg.vae_latent_channels = c.latent_channels
+        return cfg
+
+    def load_state_dict(self, state_dict, *a, **k):
+        """Also accepts the mid-block attention names written before diffusers 0.14 (query / key / value / proj_attn)."""
+        return super().load_state_dict(_convert_legacy_vae_keys(state_dict), *a, **k)
+
+    def workspace_bytes(self, n, h, w) -> int:
+        """Device workspace of decoding n latents of h x w and of encoding n images of 8h x 8w."""
+        hd = self._sync_native()
+        f = N.lib().hv_workspace_bytes
+        f.restype = C.c_size_t
+        return int(f(hd, N.i32(n), N.i32(1), N.i32(h), N.i32(w)))
+
+    def reserve_workspace(self, n, h, w):
+        """Grow the native workspace for n latents of h x w (and n images of 8h x 8w) now, e.g. before capturing a CUDA graph."""
+        self._reserve(self._sync_native(), n, 1, h, w)
+
+    @torch.no_grad()
+    def encode(self, x: torch.Tensor, return_dict: bool = True):
+        if x.dim() != 4:
+            raise ValueError(f"Expected x to have ndim=4 (n c h w), got {x.dim()}")
+        B, Cc, H, W = x.shape
+        if Cc != self.config.in_channels:
+            raise ValueError(f"image has {Cc} channels, model expects {self.config.in_channels}")
+        if B == 0 or H % 8 or W % 8:
+            raise ValueError(f"encode needs a non-empty batch of images whose sides are multiples of 8; got {tuple(x.shape)}")
+        h = self._sync_native()
+        xin = self._as_half(x, "image")
+        moments = torch.empty((B, 2 * self.config.latent_channels, H // 8, W // 8), device=xin.device, dtype=torch.float16)
+        self._reserve(h, B, 1, H // 8, W // 8)
+        N.check(N.lib().hv_vae_encode(h, N.ptr(xin), N.ptr(moments), N.i32(B), N.i32(H), N.i32(W), None, C.c_size_t(0), N.stream()), h)
+        dist = DiagonalGaussianDistribution(moments.to(x.dtype) if x.dtype != torch.float16 else moments)
+        if not return_dict:
+            return (dist,)
+        return AutoencoderKLOutput(latent_dist=dist)
+
+    @torch.no_grad()
+    def decode(self, z: torch.Tensor, return_dict: bool = True, generator=None):
+        if z.dim() != 4:
+            raise ValueError(f"Expected z to have ndim=4 (n c h w), got {z.dim()}")
+        B, Cc, H, W = z.shape
+        if Cc != self.config.latent_channels:
+            raise ValueError(f"latents have {Cc} channels, model expects {self.config.latent_channels}")
+        if B == 0:
+            raise ValueError("decode needs a non-empty batch")
+        h = self._sync_native()
+        zin = self._as_half(z, "latents")
+        out = torch.empty((B, self.config.out_channels, 8 * H, 8 * W), device=zin.device, dtype=torch.float16)
+        self._reserve(h, B, 1, H, W)
+        N.check(N.lib().hv_vae_decode(h, N.ptr(zin), N.ptr(out), N.i32(B), N.i32(H), N.i32(W), None, C.c_size_t(0), N.stream()), h)
+        out = out.to(z.dtype) if z.dtype != torch.float16 else out
+        if not return_dict:
+            return (out,)
+        return DecoderOutput(sample=out)
+
+    def forward(self, sample: torch.Tensor, sample_posterior: bool = False, return_dict: bool = True, generator=None):
+        if sample_posterior:
+            raise NotImplementedError("sampling the posterior is not implemented (inference uses its mean)")
+        return self.decode(self.encode(sample).latent_dist.mode(), return_dict=return_dict)
+
+    @classmethod
+    def from_pretrained(cls, pretrained_model_path, subfolder=None, torch_dtype=None, **kwargs):
+        """diffusers-style loader: ``<path>[/<subfolder>]/config.json`` + ``diffusion_pytorch_model.safetensors`` (or ``.bin``); old
+        attention names are converted.  Builds on the CPU; move it with ``.to("cuda", torch.float16)``."""
+        path = os.path.join(str(pretrained_model_path), subfolder) if subfolder is not None else str(pretrained_model_path)
+        with open(os.path.join(path, "config.json")) as f:
+            cfg = {k: v for k, v in json.load(f).items() if not k.startswith("_")}
+        import inspect
+
+        allowed = set(inspect.signature(cls.__init__).parameters) - {"self", "unused"}
+        model = cls(**{k: v for k, v in cfg.items() if k in allowed})
+        st_path = os.path.join(path, "diffusion_pytorch_model.safetensors")
+        if os.path.exists(st_path):
+            from safetensors.torch import load_file
+
+            state = load_file(st_path, device="cpu")
+        else:
+            bin_path = os.path.join(path, "diffusion_pytorch_model.bin")
+            if not os.path.isfile(bin_path):
+                raise FileNotFoundError(f"no weights file found in {path}")
+            state = torch.load(bin_path, map_location="cpu", weights_only=True)
+        missing = model.load_state_dict(state, strict=False).missing_keys
+        if missing:
+            raise RuntimeError(f"{path}: weights missing from the checkpoint: {missing[:5]}{' ...' if len(missing) > 5 else ''}")
+        if torch_dtype is not None:
+            model = model.to(torch_dtype)
+        return model

@@ -8,6 +8,8 @@
  *   HV_KIND_CAMERA_ENCODER CameraPoseEncoder.forward     src/cameractrl/pose_adaptor.py:232-248
  *   hv_set_ref_bank / hv_clear_ref_banks                 ReferenceAttentionControl.update / .clear
  *                                                        src/models/mutual_self_attention.py:302-363
+ *   HV_KIND_VAE           AutoencoderKL.encode / .decode (diffusers 0.24, the SD layout configs/prompts/stage2.yaml points at):
+ *                         what Pose2VideoPipeline / Pose2ImagePipeline call for the reference latents and the output frames
  *   HV_KIND_UNET2D_REF    UNet2DConditionModel.forward in "write" mode (the reference / "writer" UNet, once per clip)
  *                                                        src/models/unet_2d_condition.py:872-1308 (post-process removed
  *                                                        :1295-1299), write hook mutual_self_attention.py:137-146
@@ -30,7 +32,7 @@ extern "C" {
 
 typedef struct hv_model* hv_handle;
 
-enum hv_kind { HV_KIND_UNET3D = 0, HV_KIND_POSE_GUIDER = 1, HV_KIND_CAMERA_ENCODER = 2, HV_KIND_UNET2D_REF = 3 };
+enum hv_kind { HV_KIND_UNET3D = 0, HV_KIND_POSE_GUIDER = 1, HV_KIND_CAMERA_ENCODER = 2, HV_KIND_UNET2D_REF = 3, HV_KIND_VAE = 4 };
 enum hv_dtype { HV_F16 = 0, HV_F32 = 1 };
 enum hv_forward_flags {
   HV_FLAG_CFG = 1,         /* batch = [uncond half ; cond half]: the first half ignores the reference banks
@@ -63,6 +65,9 @@ typedef struct hv_config {
   int32_t cam_nums_rb;           /* 2 */
   int32_t cam_heads;             /* 8 */
   int32_t cam_max_len;           /* 24 */
+  /* AutoencoderKL (diffusers 0.24, SD layout): block_out_channels (128 256 512 512), norm_groups (32), in_channels /
+   * out_channels (3 image channels) above, and: */
+  int32_t vae_latent_channels;   /* 4 */
 } hv_config;
 
 int hv_create(const hv_config* cfg, hv_handle* out);
@@ -118,6 +123,18 @@ int hv_camera_encoder_forward(hv_handle h, const void* plucker, void* out, int32
  * scripts/pose2vid.py:66-80 hands to ray_condition.  The embedding is generated inside the PixelUnshuffle producer. */
 int hv_camera_encoder_forward_rays(hv_handle h, const float* intrinsics, const float* c2w, void* out, int32_t B, int32_t F, int32_t H,
                                    int32_t W, void* workspace, size_t ws_bytes, hv_stream_t stream);
+
+/* AutoencoderKL (kind HV_KIND_VAE; weights under diffusers' key names: encoder.*, decoder.*, quant_conv, post_quant_conv, the mid-block
+ * attention as mid_block.attentions.0.{group_norm,to_q,to_k,to_v,to_out.0}).
+ * hv_vae_decode: z (N, latent, h, w) -> out (N, out_channels, 8h, 8w), post_quant_conv included; the 1/scaling_factor stays with the caller.
+ * hv_vae_encode: x (N, in_channels, H, W), H and W multiples of 8 -> moments (N, 2*latent, H/8, W/8) = [mean | logvar], quant_conv included.
+ * Every frame is computed independently of the others in the call.  For this kind hv_workspace_bytes(h, N, 1, h, w) and
+ * hv_reserve_workspace(h, N, 1, h, w) take the LATENT size: the workspace covers both decoding N latents of h x w and encoding N images of
+ * 8h x 8w.  Like the other forwards these never allocate or synchronise (CUDA-graph capturable after hv_reserve_workspace). */
+int hv_vae_decode(hv_handle h, const void* z, void* out, int32_t N, int32_t height, int32_t width, void* workspace, size_t ws_bytes,
+                  hv_stream_t stream);
+int hv_vae_encode(hv_handle h, const void* x, void* moments, int32_t N, int32_t H, int32_t W, void* workspace, size_t ws_bytes,
+                  hv_stream_t stream);
 
 /* Debug taps (per-layer error ladder, scripts/error_ladder.py): the activation leaving the i-th block of the UNet forward (conv_in, every
  * resnet / transformer / motion module / down- / up-sampler, in execution order) is copied to dst[i] as channels-last fp16

@@ -12,6 +12,8 @@
  *   hv_op_attention       F.scaled_dot_product_attention over the spatial tokens of a frame, optional reference-bank
  *                         keys (ReferenceAttentionControl read hook)  src/models/attention.py:405; mutual_self_attention.py:147-186
  *   hv_op_temporal_attention  SDPA over the frame axis per pixel   src/models/motion_module.py:351-388
+ *   hv_op_attention_d512  the one-head d = 512 attention of AutoencoderKL's mid block (diffusers Attention, vae.encode / vae.decode)
+ *   hv_op_conv3x3_s2_pad_end  AutoencoderKL's Downsample2D: F.pad(x, (0, 1, 0, 1)) + stride-2 conv
  *
  * All functions launch asynchronously on `stream`, never synchronise, return 0 on success or a negative hv_status,
  * and do not throw.  Pointers are caller-owned device memory, 16-byte aligned, row strides multiples of 8 elements.
@@ -93,6 +95,12 @@ int hv_pack_upconv2x2(const void* W, void* out, int64_t Cout, int64_t Cin, hv_st
 int hv_op_conv3x3(const void* X, const void* Wp, void* out, int64_t ldc, int64_t NF, int64_t H, int64_t W, int64_t Cin,
                   int64_t Cout, int32_t stride, const hv_epilogue* ep, hv_stream_t stream);
 
+/* AutoencoderKL's Downsample2D: F.pad(x, (0, 1, 0, 1)) then a 3x3 convolution with stride 2 and padding 0, i.e. hv_op_conv3x3 at stride 2
+ * with the padding at the bottom / right only (no padded copy is made; the rows / columns past the end read as zero).  Same X, Wp, out and
+ * epilogue conventions as hv_op_conv3x3; H and W must be even, the output is (NF, H/2, W/2, Cout). */
+int hv_op_conv3x3_s2_pad_end(const void* X, const void* Wp, void* out, int64_t ldc, int64_t NF, int64_t H, int64_t W, int64_t Cin, int64_t Cout,
+                             const hv_epilogue* ep, hv_stream_t stream);
+
 /* Small-channel direct 3x3 convolution (any Cin/Cout, stride 1/2, padding 1) for conv_in and the PoseGuider stack.
  * W is the reference layout (Cout, Cin, 3, 3) fp16; act = hv_act. */
 int hv_op_conv3x3_direct(const void* X, const void* W, const void* bias, void* out, int64_t NF, int64_t H, int64_t Wd,
@@ -122,6 +130,13 @@ int hv_op_attention(const void* Q, const void* K, const void* Vt, void* out, int
                     int32_t d, int64_t ldq, int64_t ldk, int64_t ldvt, int64_t ldo, const void* Kb, const void* Vbt,
                     int64_t Lb, int64_t ldkb, int64_t ldvbt, int64_t F, int64_t nf_nobank, int64_t vt_stride, int64_t vbt_stride,
                     hv_stream_t stream);
+
+/* Single-head attention with d = 512 (the mid-block attention of AutoencoderKL): out = softmax(Q K^T / sqrt(512)) V over the L tokens of
+ * each of NF frames, softmax statistics in fp32, P rounded to fp16 for P*V.  Q: [NF*L][ldq] and K: [NF*L][ldk] (512 columns used);
+ * Vt: [512][ldvt] = V transposed, frame n's tokens in columns [n*vt_stride, n*vt_stride + L) (vt_stride % 8 == 0, >= L; the
+ * layout hv_op_gemm_batched_b writes); out: [NF*L][ldo].  Any L >= 1. */
+int hv_op_attention_d512(const void* Q, int64_t ldq, const void* K, int64_t ldk, const void* Vt, int64_t ldvt, int64_t vt_stride, void* out,
+                         int64_t ldo, int64_t NF, int64_t L, hv_stream_t stream);
 
 /* Attention over the frame axis: tokens are rows (b, f, p) of QKV [B*F*HW][3*C] (q | k | v), one problem per
  * (b, p, head) with F <= 32 keys. out [B*F*HW][C]. */
