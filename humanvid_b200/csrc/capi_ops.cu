@@ -184,5 +184,8 @@ int hv_op_advance_index(int32_t* index, hv_stream_t stream) {
 int hv_dbg_gemm(const void* A, int64_t lda, const void* W, float* out, int64_t M, int64_t N, int64_t K, hv_stream_t stream) {
   CK(launch_dbg_gemm(H(A), lda, H(W), out, (int)M, (int)N, (int)K, ST(stream)), "hv_dbg_gemm");
 }
+int hv_dbg_gemm_plan(int64_t M, int64_t N, int64_t K, int32_t geglu, int32_t* block_n, int32_t* bst_stages, int32_t* grid) {
+  return plan_linear(M, N, K, geglu != 0, block_n, bst_stages, grid);
+}
 
 }  // extern "C"

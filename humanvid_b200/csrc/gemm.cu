@@ -311,61 +311,69 @@ void choose_conv_box(int NF, int H, int W, int* bn, int* bh, int* bw) {
   *bw = b_w;
 }
 
+// A-ring depth of the B-stationary variant, or 0 when the shape does not qualify: the BLOCK_N x K weight panel plus at least three
+// A stages must fit in shared memory, and every CTA must get at least two tiles of its n_blk.
 template <int BN>
-static cudaError_t launch_t(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const GemmProblem& p, const GemmEpilogue& e,
-                            int grid, cudaStream_t stream) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t err = cudaFuncSetAttribute(gemm_kernel<BN, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::kSmemBytes);
-    if (err != cudaSuccess) return err;
-    attr_set = true;
-  }
-  gemm_kernel<BN, false><<<grid, GEMM_THREADS, Cfg<BN>::kSmemBytes, stream>>>(a0, a1, b, p, e);
-  return cudaGetLastError();
-}
-
-// B-stationary launch; returns cudaErrorNotSupported when the shape does not qualify (caller falls back to the ring).
-template <int BN>
-static cudaError_t launch_bst(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, GemmProblem p, const GemmEpilogue& e,
-                              int m_tiles, int n_tiles, int num_sms, cudaStream_t stream) {
+static int bst_stages(int num_k_blocks, int m_tiles, int n_tiles, int num_sms) {
   using C = Cfg<BN>;
-  const int panel = p.num_k_blocks * C::kBTileBytes;
+  const int panel = num_k_blocks * C::kBTileBytes;
   int stages = (kMaxSmem - C::kFixed - panel) / A_TILE_BYTES;
   if (stages > kMaxStages) stages = kMaxStages;
   const int per_col = num_sms / n_tiles;  // CTAs sharing one n_blk
-  if (stages < 3 || per_col < 1 || m_tiles < 2 * per_col) return cudaErrorNotSupported;
+  if (stages < 3 || per_col < 1 || m_tiles < 2 * per_col) return 0;
+  return stages;
+}
+
+template <int BN, bool BST>
+static cudaError_t launch_t(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, GemmProblem p, const GemmEpilogue& e,
+                            const GemmPlan& plan, cudaStream_t stream) {
+  using C = Cfg<BN>;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t err = cudaFuncSetAttribute(gemm_kernel<BN, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
+    cudaError_t err = cudaFuncSetAttribute(gemm_kernel<BN, BST>, cudaFuncAttributeMaxDynamicSharedMemorySize, BST ? kMaxSmem : C::kSmemBytes);
     if (err != cudaSuccess) return err;
     attr_set = true;
   }
-  p.bst_stages = stages;
-  const int smem = panel + stages * A_TILE_BYTES + C::kFixed;
-  gemm_kernel<BN, true><<<per_col * n_tiles, GEMM_THREADS, smem, stream>>>(a0, a1, b, p, e);
+  p.bst_stages = plan.bst_stages;
+  const int smem = BST ? p.num_k_blocks * C::kBTileBytes + plan.bst_stages * A_TILE_BYTES + C::kFixed : C::kSmemBytes;
+  gemm_kernel<BN, BST><<<plan.grid, GEMM_THREADS, smem, stream>>>(a0, a1, b, p, e);
   return cudaGetLastError();
+}
+
+bool plan_gemm(const GemmProblem& p, int block_n, int num_sms, GemmPlan* plan) {
+  if (block_n != 128 && block_n != 160 && block_n != 256) return false;
+  const int m_tiles = p.a_mode == A_LINEAR ? (p.M + BLOCK_M - 1) / BLOCK_M : p.tiles_n * p.tiles_y * p.tiles_x * (p.a_mode == A_UPCONV2X2 ? 4 : 1);
+  const int n_tiles = p.b_batch ? p.b_batch * ((p.b_rows + block_n - 1) / block_n) : (p.N + block_n - 1) / block_n;
+  const int tiles = m_tiles * n_tiles;
+  if (tiles <= 0 || p.num_k_blocks <= 0) return false;
+  plan->bst_stages = 0;
+  plan->grid = tiles < num_sms ? tiles : num_sms;
+  if (p.a_mode == A_LINEAR && !p.b_batch && n_tiles <= num_sms) {
+    const int s = block_n == 256 ? bst_stages<256>(p.num_k_blocks, m_tiles, n_tiles, num_sms)
+                : block_n == 160 ? bst_stages<160>(p.num_k_blocks, m_tiles, n_tiles, num_sms)
+                                 : bst_stages<128>(p.num_k_blocks, m_tiles, n_tiles, num_sms);
+    if (s > 0) {
+      plan->bst_stages = s;
+      plan->grid = (num_sms / n_tiles) * n_tiles;   // gridDim.x a multiple of n_tiles: each CTA keeps one n_blk
+    }
+  }
+  return true;
 }
 
 cudaError_t launch_gemm(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const GemmProblem& p, const GemmEpilogue& e,
                         int block_n, int num_sms, cudaStream_t stream) {
-  const int m_tiles = p.a_mode == A_LINEAR ? (p.M + BLOCK_M - 1) / BLOCK_M : p.tiles_n * p.tiles_y * p.tiles_x * (p.a_mode == A_UPCONV2X2 ? 4 : 1);
-  const int n_tiles = p.b_batch ? p.b_batch * ((p.b_rows + block_n - 1) / block_n) : (p.N + block_n - 1) / block_n;
-  const int tiles = m_tiles * n_tiles;
-  if (tiles <= 0 || p.num_k_blocks <= 0) return cudaErrorInvalidValue;
+  GemmPlan plan;
+  if (!plan_gemm(p, block_n, num_sms, &plan)) return cudaErrorInvalidValue;
   if (p.b_batch && (e.bias || e.rowvec || e.residual || e.geglu || (p.b_out_stride % 8))) return cudaErrorInvalidValue;
   if (e.geglu && block_n != 256) return cudaErrorInvalidValue;
-  const int grid = tiles < num_sms ? tiles : num_sms;
-  if (p.a_mode == A_LINEAR && !p.b_batch && n_tiles <= num_sms) {
-    cudaError_t r = cudaErrorNotSupported;
-    if (block_n == 256) r = launch_bst<256>(a0, a1, b, p, e, m_tiles, n_tiles, num_sms, stream);
-    if (block_n == 160) r = launch_bst<160>(a0, a1, b, p, e, m_tiles, n_tiles, num_sms, stream);
-    if (block_n == 128) r = launch_bst<128>(a0, a1, b, p, e, m_tiles, n_tiles, num_sms, stream);
-    if (r != cudaErrorNotSupported) return r;
+  if (plan.bst_stages > 0) {
+    if (block_n == 256) return launch_t<256, true>(a0, a1, b, p, e, plan, stream);
+    if (block_n == 160) return launch_t<160, true>(a0, a1, b, p, e, plan, stream);
+    return launch_t<128, true>(a0, a1, b, p, e, plan, stream);
   }
-  if (block_n == 256) return launch_t<256>(a0, a1, b, p, e, grid, stream);
-  if (block_n == 160) return launch_t<160>(a0, a1, b, p, e, grid, stream);
-  if (block_n == 128) return launch_t<128>(a0, a1, b, p, e, grid, stream);
-  return cudaErrorInvalidValue;
+  if (block_n == 256) return launch_t<256, false>(a0, a1, b, p, e, plan, stream);
+  if (block_n == 160) return launch_t<160, false>(a0, a1, b, p, e, plan, stream);
+  return launch_t<128, false>(a0, a1, b, p, e, plan, stream);
 }
 
 }  // namespace hv

@@ -45,6 +45,16 @@ struct GemmProblem {
   int b_batch = 0, b_rows = 0, b_out_stride = 0;
 };
 
+// How launch_gemm runs a problem.  bst_stages > 0: the B-stationary variant (each CTA keeps its BLOCK_N x K weight panel in shared
+// memory and streams A through a ring of bst_stages tiles; grid is a multiple of the N tiles).  bst_stages == 0: the ring variant
+// (A and B tiles stream together), one persistent CTA per SM, grid = min(tiles, SMs).
+struct GemmPlan {
+  int bst_stages = 0;
+  int grid = 0;
+};
+// The plan launch_gemm follows for (p, block_n); false for a block_n or an empty problem it rejects.
+bool plan_gemm(const GemmProblem& p, int block_n, int num_sms, GemmPlan* plan);
+
 // C[M, N] = A[M, K] * B[N, K]^T  (fp16 in, fp32 accumulate in registers, fused epilogue, fp16 out), CTA tile 128 x block_n.
 // a0/a1: TMA maps of the A operand with 128-row boxes (see make_* helpers in tma.h), b: TMA map of the packed weights [N][K].
 // block_n must be 128, 160 or 256 (256 required for geglu); 160 = two exact tiles for the 320-wide layers.

@@ -76,6 +76,37 @@ static int pick_block_n(int64_t N, int64_t m_tiles, bool geglu, int sms) {
   return best;
 }
 
+// Problem block and tile width of the linear out[M, N] = A[M, K] W[N, K]^T: what op_gemm launches and plan_linear reports.
+static GemmProblem linear_problem(int64_t M, int64_t N, int64_t K, bool geglu, int sms, int* block_n) {
+  GemmProblem p;
+  p.M = static_cast<int>(M);
+  p.N = static_cast<int>(N);
+  p.num_k_blocks = static_cast<int>((K + 63) / 64);
+  p.a_mode = A_LINEAR;
+  *block_n = pick_block_n(N, (M + 127) / 128, geglu, sms);
+  return p;
+}
+
+int plan_linear(int64_t M, int64_t N, int64_t K, bool geglu, int* block_n, int* bst_stages, int* grid) {
+  const int sms = device_sms();
+  if (!sms) return HV_ERR_CUDA;
+  if (M <= 0 || N <= 0 || K <= 0 || M > INT32_MAX || N > INT32_MAX || K > INT32_MAX) {
+    set_error("hv_dbg_gemm_plan: bad shape M=%lld N=%lld K=%lld", (long long)M, (long long)N, (long long)K);
+    return HV_ERR_INVALID;
+  }
+  int bn;
+  const GemmProblem p = linear_problem(M, N, K, geglu, sms, &bn);
+  GemmPlan plan;
+  if (!plan_gemm(p, bn, sms, &plan)) {
+    set_error("hv_dbg_gemm_plan: no plan for M=%lld N=%lld K=%lld", (long long)M, (long long)N, (long long)K);
+    return HV_ERR_INVALID;
+  }
+  if (block_n) *block_n = bn;
+  if (bst_stages) *bst_stages = plan.bst_stages;
+  if (grid) *grid = plan.grid;
+  return HV_OK;
+}
+
 int op_gemm(const __half* A, int64_t lda, const __half* A2, int64_t lda2, int64_t K1, const __half* W, __half* out, int64_t ldc,
             int64_t M, int64_t N, int64_t K, const hv_epilogue* ep, cudaStream_t stream) {
   const int sms = device_sms();
@@ -97,18 +128,13 @@ int op_gemm(const __half* A, int64_t lda, const __half* A2, int64_t lda2, int64_
   }
   CUtensorMap ma0, ma1, mb;
   const int64_t Ka = split ? K1 : K;
-  const int64_t m_tiles = (M + 127) / 128;
-  const int bn = pick_block_n(N, m_tiles, geglu, sms);
+  int bn;
+  GemmProblem p = linear_problem(M, N, K, geglu, sms, &bn);
+  p.k_split = split ? static_cast<int>(K1 / 64) : 0;
   if (!make_map_2d(&ma0, A, M, Ka, lda, 128)) { set_error("hv_op_gemm A map: %s", tma_last_error()); return HV_ERR_TMA; }
   ma1 = ma0;
   if (split && !make_map_2d(&ma1, A2, M, K - K1, lda2, 128)) { set_error("hv_op_gemm A2 map: %s", tma_last_error()); return HV_ERR_TMA; }
   if (!make_map_2d(&mb, W, N, K, K, bn)) { set_error("hv_op_gemm W map: %s", tma_last_error()); return HV_ERR_TMA; }
-  GemmProblem p;
-  p.M = static_cast<int>(M);
-  p.N = static_cast<int>(N);
-  p.num_k_blocks = static_cast<int>((K + 63) / 64);
-  p.a_mode = A_LINEAR;
-  p.k_split = split ? static_cast<int>(K1 / 64) : 0;
   GemmEpilogue e;
   fill_epilogue(e, ep, out, ldc, N);
   cudaError_t err = launch_gemm(ma0, ma1, mb, p, e, bn, sms, stream);

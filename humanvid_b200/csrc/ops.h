@@ -14,6 +14,8 @@ void set_error(const char* fmt, ...);
 const char* last_error();
 int cuda_fail(cudaError_t e, const char* what);
 
+// The tile width and launch plan op_gemm would use for out[M, N] = A[M, K] W[N, K]^T (bst_stages 0: ring variant).
+int plan_linear(int64_t M, int64_t N, int64_t K, bool geglu, int* block_n, int* bst_stages, int* grid);
 int op_gemm(const __half* A, int64_t lda, const __half* A2, int64_t lda2, int64_t K1, const __half* W, __half* out, int64_t ldc,
             int64_t M, int64_t N, int64_t K, const hv_epilogue* ep, cudaStream_t stream);
 // out[M][n*out_stride + j] = sum_k A[M][k] * X[n][j][k] for n < batch, j < rows (X: [batch][rows][ldx]); out_stride % 8 == 0.

@@ -64,7 +64,9 @@ int hv_op_gemm(const void* A, int64_t lda, const void* A2, int64_t lda2, int64_t
                int64_t M, int64_t N, int64_t K, const hv_epilogue* ep, hv_stream_t stream);
 
 /* out[M][n*out_stride + j] = sum_k A[M][k] * X[n][j][k], n < batch, j < rows: the "swapped" GEMM that yields V^T with every
- * frame's token segment starting on a 16-byte boundary (out_stride % 8 == 0), as TMA readers of V^T require. */
+ * frame's token segment starting on a 16-byte boundary (out_stride % 8 == 0), as TMA readers of V^T require.  The pad columns
+ * [rows, round8(rows)) of each segment are written too, as 0 + rowbias[m] (0 without rowbias); columns [round8(rows), out_stride)
+ * and [batch*out_stride, ldc) are left untouched. */
 int hv_op_gemm_batched_b(const void* A, int64_t lda, const void* X, int64_t ldx, void* out, int64_t ldc, int64_t M, int64_t batch,
                          int64_t rows, int64_t out_stride, int64_t K, const void* rowbias /* fp16 [M] added to row m, or NULL */,
                          hv_stream_t stream);
@@ -106,7 +108,8 @@ int hv_op_conv3x3_s2_pad_end(const void* X, const void* Wp, void* out, int64_t l
 int hv_op_conv3x3_direct(const void* X, const void* W, const void* bias, void* out, int64_t NF, int64_t H, int64_t Wd,
                          int64_t Cin, int64_t Cout, int32_t stride, int32_t act, const void* add, hv_stream_t stream);
 
-/* GroupNorm over (H*W, C/groups) per frame, fp32 statistics; optional SiLU; reads the channel concatenation of X
+/* GroupNorm over (H*W, C/groups) per frame, fp32 statistics (summed relative to one input value of the group, so a large mean does not
+ * cancel the variance); optional SiLU; reads the channel concatenation of X
  * (C1 channels) and X2 (C2 channels, may be NULL/0) and writes one (NF, HW, C1+C2) tensor. stats: fp32 scratch
  * of hv_groupnorm_scratch_floats(...) floats (per-slab partial sums; the reduction is atomics-free and deterministic). */
 size_t hv_groupnorm_scratch_floats(int64_t C, int64_t NF, int64_t HW, int32_t groups);
@@ -191,6 +194,10 @@ int hv_pack_heads(const void* W, void* out, int32_t heads, int32_t d, int32_t dp
 
 /* Debug cross-checks (slow CUDA-core kernels, used by tests to localise a fault on the device). */
 int hv_dbg_gemm(const void* A, int64_t lda, const void* W, float* out, int64_t M, int64_t N, int64_t K, hv_stream_t stream);
+/* The launch hv_op_gemm makes for an M x N x K linear on this device (the same host function decides both): the CTA tile width
+ * *block_n (128, 160 or 256), *bst_stages > 0 for the B-stationary variant (the CTA's N x K weight panel stays in shared memory and
+ * A streams through that many stages) or 0 for the ring variant, and the persistent *grid.  Launches nothing. */
+int hv_dbg_gemm_plan(int64_t M, int64_t N, int64_t K, int32_t geglu, int32_t* block_n, int32_t* bst_stages, int32_t* grid);
 
 const char* hv_ops_last_error(void);
 int hv_num_sms(void);
