@@ -28,7 +28,7 @@ class Epilogue(C.Structure):
     ]
 
 
-ACT_NONE, ACT_RELU, ACT_SILU = 0, 1, 2
+ACT_NONE, ACT_RELU, ACT_SILU, ACT_QUICK_GELU = 0, 1, 2, 3
 
 
 def lib() -> C.CDLL:

@@ -376,6 +376,7 @@ cudaError_t launch_attention(const AttnArgs& a, int /*num_sms*/, cudaStream_t st
     case 16: return launch_attn_t<16>(a, stream);
     case 32: return launch_attn_t<32>(a, stream);
     case 40: return launch_attn_t<40>(a, stream);
+    case 64: return launch_attn_t<64>(a, stream);
     case 80: return launch_attn_t<80>(a, stream);
     case 160: return launch_attn_t<160>(a, stream);
     default: return cudaErrorInvalidValue;

@@ -61,6 +61,16 @@ int hv_op_pose_conv_in(const void* X, const void* W, const void* bias, void* out
   CK(launch_pg_conv_in(H(X), H(W), H(bias), HM(out), (int)B, (int)F, (int)Hh, (int)Wd, act, device_sms(), ST(stream)), "hv_op_pose_conv_in");
 }
 
+int hv_op_clip_patchify(const void* X, void* out, int64_t B, int64_t Cc, int64_t S, int64_t p, int64_t Kpad, hv_stream_t stream) {
+  if (!device_sms()) return HV_ERR_CUDA;
+  if (!X || !out || B <= 0 || Cc <= 0 || p <= 0 || S <= 0 || (S % p) || (Kpad % 8) || Kpad < Cc * p * p || B * S * S * Cc > INT32_MAX) {
+    set_error("hv_op_clip_patchify: bad shape B=%lld C=%lld S=%lld p=%lld Kpad=%lld (S %% p == 0, Kpad >= C p^2 and a multiple of 8)", (long long)B,
+              (long long)Cc, (long long)S, (long long)p, (long long)Kpad);
+    return HV_ERR_INVALID;
+  }
+  CK(launch_clip_patchify(H(X), HM(out), (int)B, (int)Cc, (int)S, (int)p, (int)Kpad, device_sms(), ST(stream)), "hv_op_clip_patchify");
+}
+
 int hv_op_conv3x3_direct(const void* X, const void* W, const void* bias, void* out, int64_t NF, int64_t Hh, int64_t Wd,
                          int64_t Cin, int64_t Cout, int32_t stride, int32_t act, const void* add, hv_stream_t stream) {
   if (!device_sms()) return HV_ERR_CUDA;

@@ -256,6 +256,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ 
             } else if (e.act == ACT_SILU) {
               v0 = silu_f(v0);
               v1 = silu_f(v1);
+            } else if (e.act == ACT_QUICK_GELU) {
+              v0 = quick_gelu_f(v0);
+              v1 = quick_gelu_f(v1);
             }
             if (res != nullptr) {
               const float2 t = ldh2(res + col);

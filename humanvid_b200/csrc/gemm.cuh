@@ -10,7 +10,7 @@ namespace hv {
 // A_CONV3X3_S2_END: stride 2 with the padding (0, 1, 0, 1) of F.pad + conv2d(stride=2, padding=0) (AutoencoderKL's Downsample2D):
 // output (yo, xo) reads input rows 2 yo .. 2 yo + 2 and columns 2 xo .. 2 xo + 2, the ones past the end reading zero.
 enum AMode : int { A_LINEAR = 0, A_CONV3X3 = 1, A_CONV3X3_S2 = 2, A_UPCONV2X2 = 3, A_CONV3X3_S2_END = 4 };
-enum Act : int { ACT_NONE = 0, ACT_RELU = 1, ACT_SILU = 2 };
+enum Act : int { ACT_NONE = 0, ACT_RELU = 1, ACT_SILU = 2, ACT_QUICK_GELU = 3 };
 
 struct GemmEpilogue {
   __half* out = nullptr;           // [rows][ldc] fp16

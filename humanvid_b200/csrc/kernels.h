@@ -11,6 +11,9 @@ size_t groupnorm_scratch_floats(int C, int NF, int HW, int groups);
 cudaError_t launch_layernorm(const __half* x, const __half* gamma, const __half* beta, __half* out, long long rows, int C, float eps,
                              const __half* pre_add, long long rows_per_group, __half* x_out, const __half* pe, int hw, int F,
                              cudaStream_t stream);
+// CLIP vision embeddings: row (b, t) of B x L tokens = LayerNorm((t == 0 ? cls : patch[b * (L - 1) + t - 1]) + pos[t]); rows = B * L.
+cudaError_t launch_clip_embed_ln(const __half* patch, const __half* cls, const __half* pos, const __half* gamma, const __half* beta, __half* out,
+                                 long long rows, int L, int C, float eps, cudaStream_t stream);
 cudaError_t launch_temporal_attention(const __half* qkv, __half* out, int B, int F, int HW, int heads, int d, cudaStream_t stream);
 
 struct AttnArgs {
@@ -43,6 +46,8 @@ cudaError_t launch_conv3x3_direct_padded(const __half* x, const __half* w, const
 cudaError_t launch_pack_upconv2x2(const __half* w, __half* out, int Cout, int Cin, int num_sms, cudaStream_t s);
 cudaError_t launch_pack_geglu(const __half* w, __half* out, int rows, int K, int num_sms, cudaStream_t s);
 cudaError_t launch_pack_heads(const __half* w, __half* out, int heads, int d, int dpad, int K, int num_sms, cudaStream_t s);
+// pixels (B, Cin, S, S) -> [B * (S/p)^2][Kpad] patch rows, k = c p^2 + ky p + kx, pad columns zero (see hv_op_clip_patchify)
+cudaError_t launch_clip_patchify(const __half* x, __half* out, int B, int Cin, int S, int p, int Kpad, int num_sms, cudaStream_t s);
 // ---- small-channel convolutions of the PoseGuider front (smallconv.cu)
 bool smallconv_supported(int cin, int cout, int stride);
 cudaError_t launch_smallconv(const __half* x, const __half* wp, const __half* bias, __half* out, int NF, int H, int W, int cin, int cout, int stride,

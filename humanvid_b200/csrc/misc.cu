@@ -1,6 +1,6 @@
 // Glue kernels of the denoising path: layout changes at the (B,C,F,H,W) boundary, pixel unshuffle and the Plucker producer of
 // the camera encoder, the tiny linears of the time embedding / cross-attention collapse, the timestep embedding, small-channel
-// direct convolutions (PoseGuider conv_in), weight packing, and a slow CUDA-core GEMM used only to localise faults in tests.
+// direct convolutions (PoseGuider conv_in), CLIP's patchify, weight packing, and a slow CUDA-core GEMM used only to localise faults in tests.
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -258,9 +258,36 @@ __global__ void pack_upconv2x2_kernel(const __half* __restrict__ w, __half* __re
   }
 }
 
+// Conv2d(Cin, hidden, p, stride=p) as the A operand of a GEMM: pixels (B, Cin, S, S) -> rows (b, gy, gx) of [B * g * g][Kpad], g = S / p,
+// column k = c p^2 + ky p + kx = pixels[b][c][gy p + ky][gx p + kx] (the flattening of the conv weight), columns [Cin p^2, Kpad) zero.
+__global__ void clip_patchify_kernel(const __half* __restrict__ x, __half* __restrict__ out, long long total, int Cin, int S, int p, int Kpad) {
+  const int g = S / p, K = Cin * p * p;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total; i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int k = static_cast<int>(i % Kpad);
+    long long r = i / Kpad;
+    const int gx = static_cast<int>(r % g);
+    r /= g;
+    const int gy = static_cast<int>(r % g);
+    const long long b = r / g;
+    __half v = __float2half_rn(0.f);
+    if (k < K) {
+      const int c = k / (p * p), rem = k - c * p * p, ky = rem / p, kx = rem - ky * p;
+      v = x[((b * Cin + c) * S + gy * p + ky) * static_cast<long long>(S) + gx * p + kx];
+    }
+    out[i] = v;
+  }
+}
+
 }  // namespace
 
 #define HV_LAUNCH_CHECK() return cudaGetLastError()
+
+cudaError_t launch_clip_patchify(const __half* x, __half* out, int B, int Cin, int S, int p, int Kpad, int num_sms, cudaStream_t s) {
+  if (B <= 0 || Cin <= 0 || p <= 0 || S <= 0 || S % p || Kpad < Cin * p * p) return cudaErrorInvalidValue;
+  const long long total = static_cast<long long>(B) * (S / p) * (S / p) * Kpad;
+  clip_patchify_kernel<<<blocks_for(total, num_sms), kThreads, 0, s>>>(x, out, total, Cin, S, p, Kpad);
+  HV_LAUNCH_CHECK();
+}
 
 cudaError_t launch_ncfhw_to_nhwc(const void* x, __half* out, int B, int C, int F, int H, int W, int src_fp32, cudaStream_t s, int ldo) {
   if (ldo <= 0) ldo = C;

@@ -1,6 +1,6 @@
 // Network runtime behind include/hv_b200.h: weight ingestion under the reference's state_dict keys, packing into
 // kernel layouts, a stack-allocated activation workspace, and the forwards (UNet3DConditionModel, PoseGuider,
-// CameraPoseEncoder, AutoencoderKL encode / decode) expressed as sequences of the operators in ops.h / kernels.h.
+// CameraPoseEncoder, AutoencoderKL encode / decode, CLIPVisionModelWithProjection) expressed as sequences of the operators in ops.h / kernels.h.
 //
 // Activations are channels-last fp16 (N = B*F frames, H, W, C) == a [tokens][C] matrix, so the reference's
 // "b c f h w -> (b f) c h w", "(bf) c h w -> (bf) (hw) c" and "(b f) d c -> (b d) f c" rearranges never touch memory:
@@ -142,6 +142,14 @@ struct VaeAttnW {   // AutoencoderKL mid-block attention: one head of C = 512 ch
   __half* bv = nullptr;
   Lin out;
 };
+struct ClipLayerW {   // CLIPEncoderLayer: pre-LN self-attention (heads of d = 64, biased q / k / v) and a quick-GELU MLP
+  Norm ln1, ln2;
+  Mat wqk;            // [2 * hidden][hidden]: q_proj rows then k_proj rows (d = 64 needs no head padding)
+  __half* bqk = nullptr;
+  Mat wv;             // [heads * dv][hidden]: v_proj rows of head h at h * dv, zero rows elsewhere (dv = 80)
+  __half* bv = nullptr;  // [heads * dv]: v_proj's bias at h * dv + j, 1 at h * dv + 64 (the softmax-denominator row of V^T), else 0
+  Lin out, fc1, fc2;
+};
 
 // ------------------------------------------------------------------------------------------ workspace arena
 struct Arena {
@@ -269,6 +277,15 @@ struct hv_model {
   };
   VaeHalf enc, dec;
   Lin quant, post_quant;   // post_quant_conv zero-padded to [64][64]: its output is conv_in's 64-channel padded input
+  // ---- CLIPVisionModelWithProjection
+  static constexpr int kClipHeadDim = 64;
+  Lin clip_patch;          // patch_embedding flattened to [hidden][3 p^2] and zero-padded to [hidden][Kpad] (no bias)
+  __half* clip_cls = nullptr;   // class_embedding [hidden]
+  __half* clip_pos = nullptr;   // position_embedding [1 + (S/p)^2][hidden]
+  Norm clip_pre, clip_post;
+  std::vector<ClipLayerW> clip_layers;
+  Mat clip_proj;           // visual_projection [projection_dim][hidden]
+  int clip_dv = 0;
 
   ~hv_model() {
     for (void* p : owned) cudaFree(p);
@@ -392,6 +409,15 @@ struct hv_model {
     if (r.has_sc) r.sc = lin(pfx + ".conv_shortcut", cout, cin);
     return r;
   }
+  // [heads * dv]: 1 at row h * dv + d (the softmax-denominator row of every head of V^T), else 0
+  __half* vones(int heads, int dv, int d) {
+    std::vector<__half> ones(static_cast<size_t>(heads) * dv, __float2half(0.f));
+    for (int hh = 0; hh < heads; ++hh) ones[static_cast<size_t>(hh) * dv + d] = __float2half(1.f);
+    __half* p = dmalloc(static_cast<int64_t>(ones.size()));
+    ck(cudaMemcpyAsync(p, ones.data(), ones.size() * 2, cudaMemcpyHostToDevice, st), "vones upload");
+    ck(cudaStreamSynchronize(st), "vones sync");  // `ones` is a host temporary
+    return p;
+  }
   SpatialW spatial(const std::string& pfx, int C) {
     SpatialW s;
     s.name = pfx;
@@ -414,13 +440,7 @@ struct hv_model {
     s.dv = static_cast<int>(rup(s.d + 1, 16));
     s.wv = Mat{dmalloc(static_cast<int64_t>(s.heads) * s.dv * C), static_cast<int64_t>(s.heads) * s.dv, C};
     ck(launch_pack_heads(mat(b + ".attn1.to_v.weight", C, C).p, s.wv.p, s.heads, s.d, s.dv, C, sms, st), "pack v");
-    {
-      std::vector<__half> ones(static_cast<size_t>(s.heads) * s.dv, __float2half(0.f));
-      for (int hh = 0; hh < s.heads; ++hh) ones[static_cast<size_t>(hh) * s.dv + s.d] = __float2half(1.f);
-      s.vones = dmalloc(static_cast<int64_t>(ones.size()));
-      ck(cudaMemcpyAsync(s.vones, ones.data(), ones.size() * 2, cudaMemcpyHostToDevice, st), "vones upload");
-      ck(cudaStreamSynchronize(st), "vones sync");  // `ones` is a host temporary
-    }
+    s.vones = vones(s.heads, s.dv, s.d);
     s.out1 = lin(b + ".attn1.to_out.0", C, C);
     s.v2 = lin(b + ".attn2.to_v", C, cfg.cross_attention_dim, false);
     s.out2 = lin(b + ".attn2.to_out.0", C, C);
@@ -564,8 +584,8 @@ struct hv_model {
   }
 
   // ---- AutoencoderKL (diffusers 0.24 key names; SD layout: 4 levels, 2 resnets per encoder level, 3 per decoder level)
-  // [n_pad][k_pad] zero-padded copy of an [n][k] linear / 1x1 conv weight, bias zero-padded to n_pad
-  Lin padded_linear(const std::string& pfx, int n, int k, int n_pad, int k_pad) {
+  // [n_pad][k_pad] zero-padded copy of an [n][k] linear / 1x1 conv weight, bias (if any) zero-padded to n_pad
+  Lin padded_linear(const std::string& pfx, int n, int k, int n_pad, int k_pad, bool bias = true) {
     const Raw& w = get(pfx + ".weight");
     if (w.numel() != static_cast<int64_t>(n) * k) fail(HV_ERR_INVALID, "weight '%s.weight' has %lld elements, expected %d x %d", pfx.c_str(), (long long)w.numel(), n, k);
     Lin l;
@@ -573,7 +593,7 @@ struct hv_model {
     ck(cudaMemsetAsync(l.w.p, 0, static_cast<size_t>(n_pad) * k_pad * 2, st), "memset");
     ck(cudaMemcpy2DAsync(l.w.p, static_cast<size_t>(k_pad) * 2, w.p, static_cast<size_t>(k) * 2, static_cast<size_t>(k) * 2, n, cudaMemcpyDeviceToDevice, st),
        "padded weight copy");
-    l.bias = vec(pfx + ".bias", n, n_pad);
+    if (bias) l.bias = vec(pfx + ".bias", n, n_pad);
     return l;
   }
   VaeAttnW vae_attn(const std::string& pfx, int C) {
@@ -641,6 +661,54 @@ struct hv_model {
     }
     dec.norm_out = norm("decoder.conv_norm_out", ch[0], 1e-6f);
     dec.conv_out = conv3("decoder.conv_out", cfg.out_channels, ch[0]);
+  }
+
+  // ---- CLIPVisionModelWithProjection (transformers key names)
+  int clip_kpad() const { return static_cast<int>(rup(3LL * cfg.clip_patch_size * cfg.clip_patch_size, 64)); }
+  void build_clip() {
+    const int C = cfg.clip_hidden_size, heads = cfg.clip_heads, p = cfg.clip_patch_size, S = cfg.clip_image_size, I = cfg.clip_intermediate_size;
+    const float eps = cfg.clip_layer_norm_eps;
+    if (heads <= 0 || C != kClipHeadDim * heads) fail(HV_ERR_INVALID, "CLIP vision: hidden_size %d / %d heads: the head dim must be %d", C, heads, kClipHeadDim);
+    if (C > 1280) fail(HV_ERR_INVALID, "CLIP vision: hidden_size %d is above the 1280 the LayerNorm kernel holds per row", C);
+    if (p <= 0 || S <= 0 || S % p) fail(HV_ERR_INVALID, "CLIP vision: image_size %d must be a positive multiple of patch_size %d", S, p);
+    if (cfg.clip_layers <= 0 || I <= 0 || I % 8 || cfg.clip_projection_dim <= 0 || !(eps > 0.f))
+      fail(HV_ERR_INVALID, "CLIP vision: layers %d, intermediate_size %d (a multiple of 8), projection_dim %d and layer_norm_eps %g must be positive", cfg.clip_layers,
+           I, cfg.clip_projection_dim, eps);
+    const int L = (S / p) * (S / p) + 1;
+    const std::string e = "vision_model.embeddings.";
+    clip_patch = padded_linear(e + "patch_embedding", C, 3 * p * p, C, clip_kpad(), false);
+    clip_cls = vec(e + "class_embedding", C);
+    clip_pos = mat(e + "position_embedding.weight", L, C).p;
+    clip_pre = norm("vision_model.pre_layrnorm", C, eps);
+    clip_dv = static_cast<int>(rup(kClipHeadDim + 1, 16));
+    clip_layers.clear();
+    for (int i = 0; i < cfg.clip_layers; ++i) {
+      const std::string pf = "vision_model.encoder.layers." + std::to_string(i) + ".";
+      ClipLayerW w;
+      w.ln1 = norm(pf + "layer_norm1", C, eps);
+      w.ln2 = norm(pf + "layer_norm2", C, eps);
+      w.wqk = Mat{dmalloc(2LL * C * C), 2LL * C, C};
+      w.bqk = dmalloc(2LL * C);
+      const char* qk[2] = {"self_attn.q_proj", "self_attn.k_proj"};
+      for (int j = 0; j < 2; ++j) {
+        ck(cudaMemcpyAsync(w.wqk.p + static_cast<int64_t>(j) * C * C, mat(pf + qk[j] + ".weight", C, C).p, static_cast<size_t>(C) * C * 2,
+                           cudaMemcpyDeviceToDevice, st), "q/k concat");
+        ck(cudaMemcpyAsync(w.bqk + static_cast<int64_t>(j) * C, vec(pf + qk[j] + ".bias", C), static_cast<size_t>(C) * 2, cudaMemcpyDeviceToDevice, st),
+           "q/k bias concat");
+      }
+      w.wv = Mat{dmalloc(static_cast<int64_t>(heads) * clip_dv * C), static_cast<int64_t>(heads) * clip_dv, C};
+      ck(launch_pack_heads(mat(pf + "self_attn.v_proj.weight", C, C).p, w.wv.p, heads, kClipHeadDim, clip_dv, C, sms, st), "pack v");
+      // row bias of V^T: the ones rows, then v_proj's bias copied over the first d rows of every head
+      w.bv = vones(heads, clip_dv, kClipHeadDim);
+      ck(cudaMemcpy2DAsync(w.bv, static_cast<size_t>(clip_dv) * 2, vec(pf + "self_attn.v_proj.bias", C), kClipHeadDim * 2, kClipHeadDim * 2, heads,
+                           cudaMemcpyDeviceToDevice, st), "v bias pack");
+      w.out = lin(pf + "self_attn.out_proj", C, C);
+      w.fc1 = lin(pf + "mlp.fc1", I, C);
+      w.fc2 = lin(pf + "mlp.fc2", C, I);
+      clip_layers.push_back(w);
+    }
+    clip_post = norm("vision_model.post_layernorm", C, eps);
+    clip_proj = mat("visual_projection.weight", cfg.clip_projection_dim, C);
   }
 
   // ================================================================== op wrappers (no-ops while measuring)
@@ -1121,6 +1189,82 @@ struct hv_model {
     Tens y = op_conv3(hn, dec.conv_out, 1, nullptr, 1, HV_ACT_NONE, nullptr);
     launch(1, {}, [&] { ck(launch_nhwc_to_ncfhw(y.p, y.C, outp, N, cfg.out_channels, 1, y.H, y.W, st), "image output layout"); });
   }
+
+  // ================================================================== CLIPVisionModelWithProjection
+  // One CLIPEncoderLayer on the residual stream x ([B * L][hidden], image n's tokens in rows n L ..), result written to `out` (may be x):
+  // LN1 -> [Q | K] (+bias) and V^T (+bias, ones rows) -> attention over each image's L tokens -> out_proj + bias + x -> LN2 -> fc1 + bias +
+  // quick-GELU -> fc2 + bias + residual.
+  void clip_layer_fwd(const ClipLayerW& w, const Tens& x, __half* out) {
+    Scope s(ar);
+    const int C = x.C, L = x.W, heads = cfg.clip_heads;
+    const int64_t tokens = x.rows();
+    Tens n1 = op_ln(x, w.ln1, nullptr, 1, nullptr, nullptr, 1);
+    __half* qk = alloc_h(tokens * 2 * C);
+    hv_epilogue eqk{};
+    eqk.bias = w.bqk;
+    gemm(n1.p, C, nullptr, 0, 0, w.wqk, qk, 2 * C, tokens, &eqk);
+    const int64_t Lp = rup(L, 8), ldvt = static_cast<int64_t>(x.NF) * Lp, vrows = w.wv.rows;
+    __half* vt = alloc_h(vrows * ldvt);
+    launch(1, {CAT_GEMM, "gemm_vt", 2.0 * tokens * C * C, vrows, tokens, C},
+           [&] { ckop(op_gemm_batched_b(w.wv.p, C, n1.p, C, vt, ldvt, vrows, x.NF, L, Lp, C, w.bv, st), "V^T gemm"); });
+    Tens o = alloc_act(x.NF, x.H, x.W, C);
+    launch(1, {CAT_ATTN, "attn", 4.0 * L * C * static_cast<double>(x.NF) * L, x.NF, L, kClipHeadDim}, [&] {
+      AttnArgs a{};
+      a.q = qk; a.k = qk + C; a.vt = vt; a.out = o.p;
+      a.NF = x.NF; a.L = L; a.heads = heads; a.d = kClipHeadDim; a.dpad = kClipHeadDim;
+      a.ldq = 2 * C; a.ldk = 2 * C; a.ldvt = ldvt; a.ldo = C;
+      a.F = 1; a.nf_nobank = 0;
+      a.vt_stride = Lp;
+      cudaError_t e = launch_attention(a, sms, st);
+      if (e != cudaSuccess) fail(HV_ERR_CUDA, "CLIP attention: %s %s", cudaGetErrorString(e), tma_last_error());
+    });
+    Tens h1 = alloc_act(x.NF, x.H, x.W, C);
+    hv_epilogue eo{};
+    eo.bias = w.out.bias;
+    eo.residual = x.p;
+    eo.ldr = C;
+    gemm(o.p, C, nullptr, 0, 0, w.out.w, h1.p, C, tokens, &eo);
+    Tens n2 = op_ln(h1, w.ln2, nullptr, 1, nullptr, nullptr, 1);
+    Tens f = op_linear(n2, w.fc1, nullptr, HV_ACT_QUICK_GELU);
+    hv_epilogue e2{};
+    e2.bias = w.fc2.bias;
+    e2.residual = h1.p;
+    e2.ldr = C;
+    gemm(f.p, f.C, nullptr, 0, 0, w.fc2.w, out, C, tokens, &e2);
+  }
+  // pixels (B, 3, S, S) -> image_embeds (B, projection_dim) and, if lhs != nullptr, last_hidden_state (B, L, hidden).  Every operator works per
+  // token row, per (image, head) or per output element, so image i of a call does not depend on the other images.
+  void clip_forward(const __half* pix, __half* embeds, __half* lhs, int B, int S) {
+    if (B <= 0 || S != cfg.clip_image_size)
+      fail(HV_ERR_INVALID, "CLIPVisionModelWithProjection: %d images of %dx%d; the model takes a positive number of %dx%d images", B, S, S, cfg.clip_image_size,
+           cfg.clip_image_size);
+    const int C = cfg.clip_hidden_size, p = cfg.clip_patch_size, np = (S / p) * (S / p), L = np + 1, Kpad = clip_kpad();
+    // patch embedding: the stride-p conv as patchify + GEMM
+    __half* prow = alloc_h(static_cast<int64_t>(B) * np * Kpad);
+    launch(1, {}, [&] { ck(launch_clip_patchify(pix, prow, B, 3, S, p, Kpad, sms, st), "patchify"); });
+    Tens pe = alloc_act(B, 1, np, C);
+    gemm(prow, Kpad, nullptr, 0, 0, clip_patch.w, pe.p, C, pe.rows(), nullptr);
+    // [class_embedding ; patches] + position_embedding -> pre_layrnorm: the residual stream (B images x L tokens)
+    Tens x = alloc_act(B, 1, L, C);
+    launch(1, {CAT_NORM, "clip_embed_ln", 0, x.rows(), C, 0},
+           [&] { ck(launch_clip_embed_ln(pe.p, clip_cls, clip_pos, clip_pre.g, clip_pre.b, x.p, x.rows(), L, C, clip_pre.eps, st), "embeddings + pre_layrnorm"); });
+    for (size_t i = 0; i < clip_layers.size(); ++i) {
+      const bool last = i + 1 == clip_layers.size();
+      __half* dst = last && lhs != nullptr ? lhs : x.p;   // the stream is updated in place; the last layer writes the caller's last_hidden_state
+      clip_layer_fwd(clip_layers[i], x, dst);
+      x.p = dst;
+    }
+    // pooling: the class token of each image -> post_layernorm -> visual_projection (no bias)
+    Tens cls = alloc_act(B, 1, 1, C);
+    launch(1, {}, [&] {
+      ck(cudaMemcpy2DAsync(cls.p, static_cast<size_t>(C) * 2, x.p, static_cast<size_t>(L) * C * 2, static_cast<size_t>(C) * 2, B, cudaMemcpyDeviceToDevice, st),
+         "class tokens");
+    });
+    Tens pooled = op_ln(cls, clip_post, nullptr, 1, nullptr, nullptr, 1);
+    const int P = static_cast<int>(clip_proj.rows);
+    launch(1, {CAT_MISC, "", 2.0 * B * P * C},
+           [&] { ck(launch_small_linear(pooled.p, clip_proj.p, nullptr, embeds, B, P, C, HV_ACT_NONE, st), "visual_projection"); });
+  }
 };
 
 // ------------------------------------------------------------------------------------------ C ABI
@@ -1169,6 +1313,9 @@ static size_t measure(hv_model* h, int B, int F, int H, int W, uint32_t flags = 
     h->begin(nullptr, 0, true, nullptr);
     h->vae_encode(nullptr, nullptr, B, 8 * H, 8 * W);
     return std::max(dec_peak, h->ar.peak) + 4096;
+  } else if (h->cfg.kind == HV_KIND_CLIP_VISION) {   // (B, 1, S, S): B images of S x S pixels
+    if (F != 1 || H != W) fail(HV_ERR_INVALID, "CLIPVisionModelWithProjection: workspace shape (B, F, H, W) = (%d, %d, %d, %d) must be (B, 1, S, S)", B, F, H, W);
+    h->clip_forward(nullptr, nullptr, nullptr, B, H);
   } else {
     h->camera_forward(nullptr, nullptr, B, F, H, W);
   }
@@ -1198,7 +1345,7 @@ int hv_create(const hv_config* cfg, hv_handle* out) {
     m = new hv_model();
     m->cfg = *cfg;
     m->sms = sms;
-    if (cfg->kind < 0 || cfg->kind > HV_KIND_VAE) fail(HV_ERR_INVALID, "unknown kind %d", cfg->kind);
+    if (cfg->kind < 0 || cfg->kind > HV_KIND_CLIP_VISION) fail(HV_ERR_INVALID, "unknown kind %d", cfg->kind);
     if (cfg->kind == HV_KIND_UNET2D_REF && cfg->use_motion_module) fail(HV_ERR_INVALID, "the reference (writer) UNet has no motion modules");
     *out = m;
     return HV_OK;
@@ -1291,6 +1438,7 @@ int hv_finalize(hv_handle h, hv_stream_t stream) {
     if (h->cfg.kind == HV_KIND_UNET3D || h->cfg.kind == HV_KIND_UNET2D_REF) h->build_unet();
     else if (h->cfg.kind == HV_KIND_POSE_GUIDER) h->build_pose_guider();
     else if (h->cfg.kind == HV_KIND_VAE) h->build_vae();
+    else if (h->cfg.kind == HV_KIND_CLIP_VISION) h->build_clip();
     else h->build_camera();
     h->finalized = true;
   });
@@ -1452,6 +1600,17 @@ int hv_vae_encode(hv_handle h, const void* x, void* moments, int32_t N, int32_t 
       fail(HV_ERR_INVALID, "AutoencoderKL.encode: N = %d images of %dx%d: N must be > 0 and H, W positive multiples of 8", N, H, W);
     run_forward(h, HV_KIND_VAE, "AutoencoderKL", N, 1, H / 8, W / 8, 0, workspace, ws_bytes, stream,
                 [&] { h->vae_encode(static_cast<const __half*>(x), static_cast<__half*>(moments), N, H, W); });
+  });
+}
+
+int hv_clip_vision_forward(hv_handle h, const void* pixel_values, void* image_embeds, void* last_hidden_state, int32_t B, void* workspace,
+                           size_t ws_bytes, hv_stream_t stream) {
+  if (!h || !pixel_values || !image_embeds) return HV_ERR_INVALID;
+  return guard(h, [&] {
+    const int S = h->cfg.clip_image_size;
+    run_forward(h, HV_KIND_CLIP_VISION, "CLIPVisionModelWithProjection", B, 1, S, S, 0, workspace, ws_bytes, stream, [&] {
+      h->clip_forward(static_cast<const __half*>(pixel_values), static_cast<__half*>(image_embeds), static_cast<__half*>(last_hidden_state), B, S);
+    });
   });
 }
 

@@ -275,7 +275,76 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const __half* __restrict
   }
 }
 
+// ---------------------------------------------------------------- CLIP token assembly + pre_layrnorm: one 128-thread block per token row
+// Row (b, t) of the B x L tokens is x = (t == 0 ? class_embedding : patch row b * (L - 1) + t - 1) + position_embedding[t], normalised over C
+// in fp32 and written once in fp16 (the residual stream entering the first encoder layer).  Each thread holds up to 2 vectors of 8: C <= 2048.
+__device__ __forceinline__ float block_sum128(float v, float* sh) {
+#pragma unroll
+  for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
+  __syncthreads();
+  const float s = (sh[0] + sh[1]) + (sh[2] + sh[3]);
+  __syncthreads();
+  return s;
+}
+
+__global__ void __launch_bounds__(128) clip_embed_ln_kernel(const __half* __restrict__ patch, const __half* __restrict__ cls,
+                                                            const __half* __restrict__ pos, const __half* __restrict__ gamma,
+                                                            const __half* __restrict__ beta, __half* __restrict__ out, int L, int C, float eps) {
+  constexpr int MAXV = 2;
+  __shared__ float sh[4];
+  const long long row = blockIdx.x;
+  const int t = static_cast<int>(row % L);
+  const long long b = row / L;
+  const __half* src = t == 0 ? cls : patch + (b * (L - 1) + t - 1) * C;
+  const __half* pr = pos + static_cast<long long>(t) * C;
+  const int vecs = C / 8;
+  float v[MAXV][8];
+  float sum = 0.f;
+#pragma unroll
+  for (int k = 0; k < MAXV; ++k) {
+    const int vi = threadIdx.x + 128 * k;
+    if (vi < vecs) {
+      float p[8];
+      unpack8(__ldg(reinterpret_cast<const uint4*>(src + vi * 8)), v[k]);
+      unpack8(__ldg(reinterpret_cast<const uint4*>(pr + vi * 8)), p);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        v[k][j] += p[j];
+        sum += v[k][j];
+      }
+    }
+  }
+  const float mean = block_sum128(sum, sh) / C;
+  float sq = 0.f;
+#pragma unroll
+  for (int k = 0; k < MAXV; ++k)
+    if (threadIdx.x + 128 * k < vecs)
+#pragma unroll
+      for (int j = 0; j < 8; ++j) sq += (v[k][j] - mean) * (v[k][j] - mean);
+  const float rstd = rsqrtf(block_sum128(sq, sh) / C + eps);
+#pragma unroll
+  for (int k = 0; k < MAXV; ++k) {
+    const int vi = threadIdx.x + 128 * k;
+    if (vi < vecs) {
+      float gm[8], bt[8];
+      unpack8(__ldg(reinterpret_cast<const uint4*>(gamma + vi * 8)), gm);
+      unpack8(__ldg(reinterpret_cast<const uint4*>(beta + vi * 8)), bt);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) v[k][j] = (v[k][j] - mean) * rstd * gm[j] + bt[j];
+      *reinterpret_cast<uint4*>(out + row * C + vi * 8) = pack8(v[k]);
+    }
+  }
+}
+
 }  // namespace
+
+cudaError_t launch_clip_embed_ln(const __half* patch, const __half* cls, const __half* pos, const __half* gamma, const __half* beta, __half* out,
+                                 long long rows, int L, int C, float eps, cudaStream_t stream) {
+  if (C % 8 || C / 8 > 256 || L < 1 || rows <= 0 || rows % L || rows > 0x7fffffffLL) return cudaErrorInvalidValue;
+  clip_embed_ln_kernel<<<static_cast<unsigned>(rows), 128, 0, stream>>>(patch, cls, pos, gamma, beta, out, L, C, eps);
+  return cudaGetLastError();
+}
 
 // scratch floats needed by launch_groupnorm: final {mean, rstd} + per-slab partials
 // The split of a frame's rows into slabs (= the order its statistics are summed in) depends on HW only, never on the number of frames in

@@ -109,6 +109,8 @@ __device__ __forceinline__ float fast_rcp(float x) {
   return y;
 }
 __device__ __forceinline__ float silu_f(float x) { return __fdividef(x, 1.0f + __expf(-x)); }
+// x * sigmoid(1.702 x): the MLP activation of OpenAI's CLIP ViTs (transformers' "quick_gelu")
+__device__ __forceinline__ float quick_gelu_f(float x) { return __fdividef(x, 1.0f + __expf(-1.702f * x)); }
 
 // hidden * gelu_erf(gate) in fp32, erf-GELU via Abramowitz-Stegun 7.1.26 (|erf error| <= 1.5e-7, far below the fp16
 // rounding that follows): 0.5x(1 + erf(x/sqrt2)) = relu(x) - |x| * 0.5 erfc(|x|/sqrt2), the 0.5 folded into the polynomial.

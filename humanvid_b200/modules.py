@@ -11,6 +11,8 @@
     LayerNorm-1 outputs become the denoising UNet's K/V banks)
   * ``AutoencoderKL.encode / decode``  <->  diffusers 0.24 ``AutoencoderKL`` in the SD layout (sd-vae-ft-mse), what the pipelines
     call for the reference latents and the output frames
+  * ``CLIPVisionModelWithProjection``  <->  transformers' class of the same name (the image encoder of scripts/pose2vid.py:17,152),
+    whose ``image_embeds`` condition both UNets
 
 The ``nn.Module`` tree below only *holds parameters* under the reference's names (torch is plumbing: device memory,
 ``load_state_dict``, ``.to()``); none of its sub-modules' ``forward`` is ever executed.  All arithmetic happens in
@@ -350,6 +352,14 @@ class HvConfig(C.Structure):
         ("cam_heads", C.c_int32),
         ("cam_max_len", C.c_int32),
         ("vae_latent_channels", C.c_int32),
+        ("clip_hidden_size", C.c_int32),
+        ("clip_layers", C.c_int32),
+        ("clip_heads", C.c_int32),
+        ("clip_intermediate_size", C.c_int32),
+        ("clip_patch_size", C.c_int32),
+        ("clip_image_size", C.c_int32),
+        ("clip_projection_dim", C.c_int32),
+        ("clip_layer_norm_eps", C.c_float),
     ]
 
 
@@ -1246,6 +1256,204 @@ class AutoencoderKL(_NativeNet):
             state = load_file(st_path, device="cpu")
         else:
             bin_path = os.path.join(path, "diffusion_pytorch_model.bin")
+            if not os.path.isfile(bin_path):
+                raise FileNotFoundError(f"no weights file found in {path}")
+            state = torch.load(bin_path, map_location="cpu", weights_only=True)
+        missing = model.load_state_dict(state, strict=False).missing_keys
+        if missing:
+            raise RuntimeError(f"{path}: weights missing from the checkpoint: {missing[:5]}{' ...' if len(missing) > 5 else ''}")
+        if torch_dtype is not None:
+            model = model.to(torch_dtype)
+        return model
+
+
+# --------------------------------------------------------------------------------------------- CLIPVisionModelWithProjection
+class _ClipEmbeddings(_Shell):
+    def __init__(self, hidden, channels, image_size, patch_size):
+        super().__init__()
+        self.class_embedding = nn.Parameter(torch.zeros(hidden))
+        self.patch_embedding = nn.Conv2d(channels, hidden, patch_size, stride=patch_size, bias=False)
+        self.position_embedding = nn.Embedding((image_size // patch_size) ** 2 + 1, hidden)
+
+
+class _ClipAttention(_Shell):
+    def __init__(self, hidden):
+        super().__init__()
+        self.k_proj = nn.Linear(hidden, hidden)
+        self.v_proj = nn.Linear(hidden, hidden)
+        self.q_proj = nn.Linear(hidden, hidden)
+        self.out_proj = nn.Linear(hidden, hidden)
+
+
+class _ClipMLP(_Shell):
+    def __init__(self, hidden, intermediate):
+        super().__init__()
+        self.fc1 = nn.Linear(hidden, intermediate)
+        self.fc2 = nn.Linear(intermediate, hidden)
+
+
+class _ClipEncoderLayer(_Shell):
+    def __init__(self, hidden, intermediate, eps):
+        super().__init__()
+        self.self_attn = _ClipAttention(hidden)
+        self.layer_norm1 = nn.LayerNorm(hidden, eps=eps)
+        self.mlp = _ClipMLP(hidden, intermediate)
+        self.layer_norm2 = nn.LayerNorm(hidden, eps=eps)
+
+
+class _ClipEncoder(_Shell):
+    def __init__(self, hidden, intermediate, layers, eps):
+        super().__init__()
+        self.layers = nn.ModuleList([_ClipEncoderLayer(hidden, intermediate, eps) for _ in range(layers)])
+
+
+class _ClipVisionTransformer(_Shell):
+    def __init__(self, c):
+        super().__init__()
+        self.embeddings = _ClipEmbeddings(c.hidden_size, c.num_channels, c.image_size, c.patch_size)
+        self.pre_layrnorm = nn.LayerNorm(c.hidden_size, eps=c.layer_norm_eps)
+        self.encoder = _ClipEncoder(c.hidden_size, c.intermediate_size, c.num_hidden_layers, c.layer_norm_eps)
+        self.post_layernorm = nn.LayerNorm(c.hidden_size, eps=c.layer_norm_eps)
+
+
+@dataclass
+class CLIPVisionModelOutput:
+    """transformers' output class of the same name: ``image_embeds`` (B, projection_dim), ``last_hidden_state`` (B, 1 + patches, hidden)."""
+
+    image_embeds: torch.Tensor
+    last_hidden_state: torch.Tensor
+    hidden_states: Optional[tuple] = None
+    attentions: Optional[tuple] = None
+
+    def __getitem__(self, i):
+        return self.to_tuple()[i]
+
+    def to_tuple(self):
+        return (self.image_embeds, self.last_hidden_state)
+
+
+class CLIPVisionModelWithProjection(_NativeNet):
+    """Drop-in for ``transformers.CLIPVisionModelWithProjection`` (the pipelines' image encoder): ``CLIPVisionConfig``'s keyword names and
+    defaults, the same ``state_dict`` keys, ``from_pretrained``, and ``model(pixel_values).image_embeds`` / ``.last_hidden_state``.  The forward
+    runs on libhv_b200 (``hv_clip_vision_forward``); every image of a batch is computed independently of the others.  OpenAI CLIP ViTs are
+    supported: quick-GELU MLPs, heads of dimension 64, RGB input.  Inference only.
+    """
+
+    _kind = 5
+
+    def __init__(
+        self,
+        hidden_size: int = 768,
+        intermediate_size: int = 3072,
+        projection_dim: int = 512,
+        num_hidden_layers: int = 12,
+        num_attention_heads: int = 12,
+        num_channels: int = 3,
+        image_size: int = 224,
+        patch_size: int = 32,
+        hidden_act: str = "quick_gelu",
+        layer_norm_eps: float = 1e-5,
+        attention_dropout: float = 0.0,
+        initializer_range: float = 0.02,
+        initializer_factor: float = 1.0,
+        **unused,
+    ):
+        super().__init__()
+        unsupported = []
+        if hidden_act != "quick_gelu":
+            unsupported.append(f"hidden_act {hidden_act!r} (quick_gelu)")
+        if num_attention_heads <= 0 or hidden_size != 64 * num_attention_heads:
+            unsupported.append(f"head dim hidden_size / num_attention_heads = {hidden_size} / {num_attention_heads} (64)")
+        if hidden_size > 1280:
+            unsupported.append(f"hidden_size {hidden_size} (<= 1280)")
+        if intermediate_size <= 0 or intermediate_size % 8:
+            unsupported.append(f"intermediate_size {intermediate_size} (a positive multiple of 8)")
+        if num_channels != 3:
+            unsupported.append(f"num_channels {num_channels} (3)")
+        if patch_size <= 0 or image_size <= 0 or image_size % patch_size:
+            unsupported.append(f"image_size {image_size} not a multiple of patch_size {patch_size}")
+        if unsupported:
+            raise NotImplementedError("humanvid_b200.CLIPVisionModelWithProjection implements OpenAI CLIP ViTs only; unsupported: " + "; ".join(unsupported))
+        self.config = SimpleNamespace(hidden_size=hidden_size, intermediate_size=intermediate_size, projection_dim=projection_dim,
+                                      num_hidden_layers=num_hidden_layers, num_attention_heads=num_attention_heads, num_channels=num_channels,
+                                      image_size=image_size, patch_size=patch_size, hidden_act=hidden_act, layer_norm_eps=layer_norm_eps,
+                                      attention_dropout=attention_dropout, initializer_range=initializer_range,
+                                      initializer_factor=initializer_factor, model_type="clip_vision_model")
+        self.vision_model = _ClipVisionTransformer(self.config)
+        self.visual_projection = nn.Linear(hidden_size, projection_dim, bias=False)
+
+    def _hv_config(self):
+        c = self.config
+        cfg = HvConfig()
+        cfg.kind = 5
+        cfg.clip_hidden_size, cfg.clip_layers, cfg.clip_heads = c.hidden_size, c.num_hidden_layers, c.num_attention_heads
+        cfg.clip_intermediate_size, cfg.clip_patch_size, cfg.clip_image_size = c.intermediate_size, c.patch_size, c.image_size
+        cfg.clip_projection_dim, cfg.clip_layer_norm_eps = c.projection_dim, c.layer_norm_eps
+        return cfg
+
+    def load_state_dict(self, state_dict, *a, **k):
+        """Also accepts checkpoints that carry the ``position_ids`` buffer older transformers versions saved."""
+        return super().load_state_dict({n: v for n, v in state_dict.items() if not n.endswith("embeddings.position_ids")}, *a, **k)
+
+    def workspace_bytes(self, batch) -> int:
+        """Device workspace of one forward over `batch` images."""
+        hd = self._sync_native()
+        f = N.lib().hv_workspace_bytes
+        f.restype = C.c_size_t
+        s = self.config.image_size
+        return int(f(hd, N.i32(batch), N.i32(1), N.i32(s), N.i32(s)))
+
+    def reserve_workspace(self, batch):
+        """Grow the native workspace for `batch` images now, e.g. before capturing a CUDA graph."""
+        s = self.config.image_size
+        self._reserve(self._sync_native(), batch, 1, s, s)
+
+    @torch.no_grad()
+    def forward(self, pixel_values: torch.Tensor, output_attentions: Optional[bool] = None, output_hidden_states: Optional[bool] = None,
+                interpolate_pos_encoding: bool = False, return_dict: Optional[bool] = None):
+        if output_attentions or output_hidden_states:
+            raise NotImplementedError("humanvid_b200.CLIPVisionModelWithProjection returns image_embeds and last_hidden_state only "
+                                      "(output_attentions / output_hidden_states are not implemented)")
+        if interpolate_pos_encoding:
+            raise NotImplementedError("interpolate_pos_encoding=True is not implemented (the model takes image_size x image_size pixels)")
+        c = self.config
+        if pixel_values.dim() != 4 or pixel_values.shape[1] != c.num_channels:
+            raise ValueError(f"pixel_values must be (batch, {c.num_channels}, height, width), got {tuple(pixel_values.shape)}")
+        B, _, H, W = pixel_values.shape
+        if H != c.image_size or W != c.image_size:
+            raise ValueError(f"Input image size ({H}*{W}) doesn't match model ({c.image_size}*{c.image_size}).")
+        if B == 0:
+            raise ValueError("pixel_values is an empty batch")
+        h = self._sync_native()
+        pix = self._as_half(pixel_values, "pixel_values")
+        embeds = torch.empty((B, c.projection_dim), device=pix.device, dtype=torch.float16)
+        hidden = torch.empty((B, (c.image_size // c.patch_size) ** 2 + 1, c.hidden_size), device=pix.device, dtype=torch.float16)
+        self._reserve(h, B, 1, c.image_size, c.image_size)
+        N.check(N.lib().hv_clip_vision_forward(h, N.ptr(pix), N.ptr(embeds), N.ptr(hidden), N.i32(B), None, C.c_size_t(0), N.stream()), h)
+        if self.dtype != torch.float16:
+            embeds, hidden = embeds.to(self.dtype), hidden.to(self.dtype)
+        if return_dict is False:
+            return (embeds, hidden)
+        return CLIPVisionModelOutput(image_embeds=embeds, last_hidden_state=hidden)
+
+    @classmethod
+    def from_pretrained(cls, pretrained_model_path, subfolder=None, torch_dtype=None, **kwargs):
+        """transformers-style loader: ``<path>[/<subfolder>]/config.json`` (a ``clip_vision_model`` config) + ``model.safetensors`` (or
+        ``pytorch_model.bin``).  Builds on the CPU; move it with ``.to("cuda", torch.float16)``."""
+        path = os.path.join(str(pretrained_model_path), subfolder) if subfolder is not None else str(pretrained_model_path)
+        with open(os.path.join(path, "config.json")) as f:
+            cfg = {k: v for k, v in json.load(f).items() if not k.startswith("_")}
+        import inspect
+
+        allowed = set(inspect.signature(cls.__init__).parameters) - {"self", "unused"}
+        model = cls(**{k: v for k, v in cfg.items() if k in allowed})
+        st_path = os.path.join(path, "model.safetensors")
+        if os.path.exists(st_path):
+            from safetensors.torch import load_file
+
+            state = load_file(st_path, device="cpu")
+        else:
+            bin_path = os.path.join(path, "pytorch_model.bin")
             if not os.path.isfile(bin_path):
                 raise FileNotFoundError(f"no weights file found in {path}")
             state = torch.load(bin_path, map_location="cpu", weights_only=True)

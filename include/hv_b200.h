@@ -13,6 +13,8 @@
  *   HV_KIND_UNET2D_REF    UNet2DConditionModel.forward in "write" mode (the reference / "writer" UNet, once per clip)
  *                                                        src/models/unet_2d_condition.py:872-1308 (post-process removed
  *                                                        :1295-1299), write hook mutual_self_attention.py:137-146
+ *   HV_KIND_CLIP_VISION   transformers' CLIPVisionModelWithProjection.forward (the image encoder whose image_embeds condition both UNets,
+ *                         scripts/pose2vid.py:17,152)
  *
  * Contract: all tensor arguments are caller-owned CUDA device pointers (torch allocations), contiguous, fp16 unless
  * stated, in the reference's own layouts ((B,C,F,H,W) etc.).  The library owns only its packed weights, reference
@@ -32,7 +34,7 @@ extern "C" {
 
 typedef struct hv_model* hv_handle;
 
-enum hv_kind { HV_KIND_UNET3D = 0, HV_KIND_POSE_GUIDER = 1, HV_KIND_CAMERA_ENCODER = 2, HV_KIND_UNET2D_REF = 3, HV_KIND_VAE = 4 };
+enum hv_kind { HV_KIND_UNET3D = 0, HV_KIND_POSE_GUIDER = 1, HV_KIND_CAMERA_ENCODER = 2, HV_KIND_UNET2D_REF = 3, HV_KIND_VAE = 4, HV_KIND_CLIP_VISION = 5 };
 enum hv_dtype { HV_F16 = 0, HV_F32 = 1 };
 enum hv_forward_flags {
   HV_FLAG_CFG = 1,         /* batch = [uncond half ; cond half]: the first half ignores the reference banks
@@ -68,6 +70,16 @@ typedef struct hv_config {
   /* AutoencoderKL (diffusers 0.24, SD layout): block_out_channels (128 256 512 512), norm_groups (32), in_channels /
    * out_channels (3 image channels) above, and: */
   int32_t vae_latent_channels;   /* 4 */
+  /* CLIPVisionModelWithProjection (transformers CLIPVisionConfig; ViT-L/14 values shown).  Head dim hidden / heads must be 64, the MLP
+   * activation is quick_gelu, 3 image channels. */
+  int32_t clip_hidden_size;       /* 1024 */
+  int32_t clip_layers;            /* num_hidden_layers = 24 */
+  int32_t clip_heads;             /* num_attention_heads = 16 */
+  int32_t clip_intermediate_size; /* 4096 */
+  int32_t clip_patch_size;        /* 14 */
+  int32_t clip_image_size;        /* 224 */
+  int32_t clip_projection_dim;    /* 768 */
+  float clip_layer_norm_eps;      /* 1e-5 */
 } hv_config;
 
 int hv_create(const hv_config* cfg, hv_handle* out);
@@ -135,6 +147,15 @@ int hv_vae_decode(hv_handle h, const void* z, void* out, int32_t N, int32_t heig
                   hv_stream_t stream);
 int hv_vae_encode(hv_handle h, const void* x, void* moments, int32_t N, int32_t H, int32_t W, void* workspace, size_t ws_bytes,
                   hv_stream_t stream);
+
+/* CLIPVisionModelWithProjection (kind HV_KIND_CLIP_VISION; weights under transformers' key names: vision_model.embeddings.*,
+ * vision_model.pre_layrnorm.*, vision_model.encoder.layers.{i}.*, vision_model.post_layernorm.*, visual_projection.weight).
+ * pixel_values (B, 3, S, S) with S = clip_image_size -> image_embeds (B, clip_projection_dim) = visual_projection(post_layernorm(class token
+ * of the last layer)), and last_hidden_state (B, 1 + (S/p)^2, clip_hidden_size) (the last encoder layer's output, without post_layernorm) unless
+ * it is NULL; all fp16.  Every image is computed independently of the others in the call.  For this kind hv_workspace_bytes(h, B, 1, S, S) and
+ * hv_reserve_workspace(h, B, 1, S, S) take the pixel size.  Never allocates or synchronises (CUDA-graph capturable after hv_reserve_workspace). */
+int hv_clip_vision_forward(hv_handle h, const void* pixel_values, void* image_embeds, void* last_hidden_state, int32_t B, void* workspace,
+                           size_t ws_bytes, hv_stream_t stream);
 
 /* Debug taps (per-layer error ladder, scripts/error_ladder.py): the activation leaving the i-th block of the UNet forward (conv_in, every
  * resnet / transformer / motion module / down- / up-sampler, in execution order) is copied to dst[i] as channels-last fp16

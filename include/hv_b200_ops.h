@@ -14,6 +14,7 @@
  *   hv_op_temporal_attention  SDPA over the frame axis per pixel   src/models/motion_module.py:351-388
  *   hv_op_attention_d512  the one-head d = 512 attention of AutoencoderKL's mid block (diffusers Attention, vae.encode / vae.decode)
  *   hv_op_conv3x3_s2_pad_end  AutoencoderKL's Downsample2D: F.pad(x, (0, 1, 0, 1)) + stride-2 conv
+ *   hv_op_clip_patchify   the patch embedding of CLIPVisionModelWithProjection (Conv2d(3, hidden, p, stride=p)) as the A operand of hv_op_gemm
  *
  * All functions launch asynchronously on `stream`, never synchronise, return 0 on success or a negative hv_status,
  * and do not throw.  Pointers are caller-owned device memory, 16-byte aligned, row strides multiples of 8 elements.
@@ -39,7 +40,8 @@ enum hv_status {
   HV_ERR_STATE = -5      /* call order violation */
 };
 
-enum hv_act { HV_ACT_NONE = 0, HV_ACT_RELU = 1, HV_ACT_SILU = 2 };
+/* HV_ACT_QUICK_GELU: x * sigmoid(1.702 x), the MLP activation of OpenAI's CLIP ViTs (hv_op_gemm / hv_op_conv3x3 epilogues only). */
+enum hv_act { HV_ACT_NONE = 0, HV_ACT_RELU = 1, HV_ACT_SILU = 2, HV_ACT_QUICK_GELU = 3 };
 
 /* Fused epilogue of hv_op_gemm / hv_op_conv3x3, applied in this order in fp32 with ONE fp16 rounding at the store (the
  * reference's eager fp16 modules round after every step; the fp32 oracle is the parity anchor):  v = acc + bias;
@@ -103,6 +105,12 @@ int hv_op_conv3x3(const void* X, const void* Wp, void* out, int64_t ldc, int64_t
 int hv_op_conv3x3_s2_pad_end(const void* X, const void* Wp, void* out, int64_t ldc, int64_t NF, int64_t H, int64_t W, int64_t Cin, int64_t Cout,
                              const hv_epilogue* ep, hv_stream_t stream);
 
+/* Patches of a stride-p, p x p convolution (CLIP's patch embedding) as the rows of a GEMM operand: X (B, C, S, S) fp16 NCHW, S % p == 0 ->
+ * out [B * (S/p)^2][Kpad], row (b, gy, gx) in raster order, column k = c p^2 + ky p + kx holding X[b][c][gy p + ky][gx p + kx]; columns
+ * [C p^2, Kpad) are written as zero.  Kpad >= C p^2 and a multiple of 8.  hv_op_gemm of this with the conv weight flattened to [hidden][C p^2]
+ * and zero-padded to [hidden][Kpad] is the convolution, one output row per patch. */
+int hv_op_clip_patchify(const void* X, void* out, int64_t B, int64_t C, int64_t S, int64_t p, int64_t Kpad, hv_stream_t stream);
+
 /* Small-channel direct 3x3 convolution (any Cin/Cout, stride 1/2, padding 1) for conv_in and the PoseGuider stack.
  * W is the reference layout (Cout, Cin, 3, 3) fp16; act = hv_act. */
 int hv_op_conv3x3_direct(const void* X, const void* W, const void* bias, void* out, int64_t NF, int64_t H, int64_t Wd,
@@ -128,7 +136,7 @@ int hv_op_layernorm(const void* X, const void* gamma, const void* beta, void* ou
  * P*V column is the softmax denominator), remaining rows zero; holding
  * V transposed: frame n's tokens occupy columns [n*vt_stride, n*vt_stride + L), vt_stride % 8 == 0.  Optional bank keys/values per batch item (frame n uses bank n / F):
  * Kb [B][Lb][ldkb], Vbt [heads*dv][B*vbt_stride] (same row layout).  Frames with n < nf_nobank attend to their own L keys only (the
- * unconditional CFG half).  out: [NF*L][heads*d]. */
+ * unconditional CFG half).  out: [NF*L][heads*d].  d is one of 8, 16, 32, 40, 64, 80, 160; other head dims return an error. */
 int hv_op_attention(const void* Q, const void* K, const void* Vt, void* out, int64_t NF, int64_t L, int32_t heads,
                     int32_t d, int64_t ldq, int64_t ldk, int64_t ldvt, int64_t ldo, const void* Kb, const void* Vbt,
                     int64_t Lb, int64_t ldkb, int64_t ldvbt, int64_t F, int64_t nf_nobank, int64_t vt_stride, int64_t vbt_stride,
