@@ -12,6 +12,7 @@
 #include <stdint.h>
 #include <stdlib.h>
 
+#include "kernels.h"
 #include "ptx.cuh"
 #include "tma.h"
 
@@ -389,42 +390,59 @@ temporal_attn_tma_kernel(const __grid_constant__ CUtensorMap map_qkv, const __gr
 }
 
 template <int D, int HPB>
-static cudaError_t launch_tt(const __half* qkv, __half* out, int B, int F, int HW, int heads, float scale_log2, cudaStream_t stream) {
+static cudaError_t launch_tt(const __half* qkv, __half* out, int B, int F, int HW, int heads, float scale_log2, unsigned grid, cudaStream_t stream) {
   using C = TTCfg<D, HPB>;
   const int Cc = heads * D;
   CUtensorMap mq, mo;
   if (!make_map_frames(&mq, qkv, static_cast<int64_t>(B) * F, HW, 3LL * Cc, 3LL * Cc, D * HPB, F)) return cudaErrorInvalidValue;
   if (!make_map_frames(&mo, out, static_cast<int64_t>(B) * F, HW, Cc, Cc, D * HPB, F)) return cudaErrorInvalidValue;
   static bool attr = false;
-  static int sms = 0;
   if (!attr) {
     cudaError_t e = cudaFuncSetAttribute(temporal_attn_tma_kernel<D, HPB>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes);
     if (e != cudaSuccess) return e;
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     attr = true;
   }
-  const long long nprob = static_cast<long long>(B) * HW * (heads / HPB);
-  long long ctas = (nprob + TT_WARPS - 1) / TT_WARPS;
-  if (ctas > sms) ctas = sms;
-  temporal_attn_tma_kernel<D, HPB><<<static_cast<unsigned>(ctas), TT_WARPS * 32, C::kSmemBytes, stream>>>(mq, mo, B, F, HW, heads, scale_log2);
+  temporal_attn_tma_kernel<D, HPB><<<grid, TT_WARPS * 32, C::kSmemBytes, stream>>>(mq, mo, B, F, HW, heads, scale_log2);
   return cudaGetLastError();
 }
 
+constexpr int kRegWarpsPerBlock = 8;
+
 }  // namespace
+
+TemporalPlan plan_temporal_attention(int B, int HW, int heads, int d, int sms) {
+  TemporalPlan p;
+  const long long nprob = static_cast<long long>(B) * HW * heads;
+  // the two high-resolution levels; small problems keep the register kernel.  The choice depends on HW only, not on the batch size
+  // (a one-half unit of the multi-GPU split must run the same kernel as that half of a CFG batch).
+  if (static_cast<long long>(HW) * heads >= 2048 && ((d == 40 && heads % 2 == 0) || d == 80)) {
+    p.tma = true;
+    p.heads_per_box = d == 40 ? 2 : 1;
+    const long long ctas = (nprob / p.heads_per_box + TT_WARPS - 1) / TT_WARPS;   // persistent: at most one CTA per SM
+    p.grid = static_cast<unsigned>(ctas < sms ? ctas : sms);
+  } else {
+    p.tma = false;
+    p.heads_per_box = 1;
+    p.grid = static_cast<unsigned>((nprob + kRegWarpsPerBlock - 1) / kRegWarpsPerBlock);
+  }
+  return p;
+}
 
 cudaError_t launch_temporal_attention(const __half* qkv, __half* out, int B, int F, int HW, int heads, int d, cudaStream_t stream) {
   if (F < 1 || F > 32) return cudaErrorInvalidValue;
-  const long long nprob = static_cast<long long>(B) * HW * heads;
-  const int wpb = 8;
-  const unsigned grid = static_cast<unsigned>((nprob + wpb - 1) / wpb);
+  static int sms = 0;
+  if (!sms) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  }
+  const TemporalPlan plan = plan_temporal_attention(B, HW, heads, d, sms);
+  const unsigned grid = plan.grid;
+  const int wpb = kRegWarpsPerBlock;
   const float scale_log2 = 1.4426950408889634f / sqrtf(static_cast<float>(d));
-  // the two high-resolution levels; small problems keep the register kernel.  The choice depends on HW only, not on the batch size
-  // (a one-half unit of the multi-GPU split must run the same kernel as that half of a CFG batch).
-  if (static_cast<long long>(HW) * heads >= 2048) {
-    if (d == 40 && heads % 2 == 0) return launch_tt<40, 2>(qkv, out, B, F, HW, heads, scale_log2, stream);
-    if (d == 80) return launch_tt<80, 1>(qkv, out, B, F, HW, heads, scale_log2, stream);
+  if (plan.tma) {
+    if (d == 40) return launch_tt<40, 2>(qkv, out, B, F, HW, heads, scale_log2, grid, stream);
+    return launch_tt<80, 1>(qkv, out, B, F, HW, heads, scale_log2, grid, stream);
   }
   switch (d) {
     case 40: temporal_attn_kernel<40><<<grid, wpb * 32, 0, stream>>>(qkv, out, B, F, HW, heads, scale_log2); break;

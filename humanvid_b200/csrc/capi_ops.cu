@@ -100,14 +100,34 @@ int hv_op_attention(const void* Q, const void* K, const void* Vt, void* out, int
                     int64_t ldq, int64_t ldk, int64_t ldvt, int64_t ldo, const void* Kb, const void* Vbt, int64_t Lb,
                     int64_t ldkb, int64_t ldvbt, int64_t F, int64_t nf_nobank, int64_t vt_stride, int64_t vbt_stride, hv_stream_t stream) {
   if (!device_sms()) return HV_ERR_CUDA;
-  AttnArgs a;
-  a.q = H(Q); a.k = H(K); a.vt = H(Vt); a.out = HM(out);
-  a.NF = (int)NF; a.L = (int)L; a.heads = heads; a.d = d; a.dpad = (d + 15) / 16 * 16;  // V^T rows per head: (d + 1 + 15) / 16 * 16, row d of every head = ones
-  a.ldq = ldq; a.ldk = ldk; a.ldvt = ldvt; a.ldo = ldo;
-  a.kb = H(Kb); a.vbt = H(Vbt); a.Lb = Kb ? (int)Lb : 0; a.ldkb = ldkb; a.ldvbt = ldvbt;
-  a.F = (int)F; a.nf_nobank = (int)nf_nobank; a.vt_stride = vt_stride; a.vbt_stride = vbt_stride;
   if ((vt_stride % 8) || (vbt_stride % 8) || vt_stride < L) { set_error("hv_op_attention: V^T frame strides must be multiples of 8 and >= L"); return HV_ERR_INVALID; }
   if ((ldq % 8) || (ldk % 8) || (ldvt % 8) || (ldo % 8) || (d % 8)) { set_error("hv_op_attention: strides / head dim must be multiples of 8"); return HV_ERR_INVALID; }
+  // every token, V^T column and TMA coordinate below is an int, and NF / heads are grid dimensions (<= 65535)
+  const bool d_ok = d == 8 || d == 16 || d == 32 || d == 40 || d == 64 || d == 80 || d == 160;
+  const int64_t dpad = (d + 15) / 16 * 16;
+  if (!Q || !K || !Vt || !out || NF < 1 || NF > 65535 || L < 1 || L > INT32_MAX || vt_stride > INT32_MAX || heads < 1 || heads > 65535 || !d_ok ||
+      NF * L > INT32_MAX || NF * vt_stride > INT32_MAX || nf_nobank < 0 || nf_nobank > NF || ldo < heads * d || ldq < heads * dpad || ldk < heads * dpad ||
+      ldvt < NF * vt_stride) {
+    set_error("hv_op_attention: bad arguments NF=%lld L=%lld heads=%d d=%d ldq=%lld ldk=%lld ldvt=%lld ldo=%lld vt_stride=%lld nf_nobank=%lld "
+              "(pointers non-NULL, 1 <= NF, heads <= 65535, 0 <= nf_nobank <= NF, ldo >= heads*d, ldq and ldk >= heads*dpad, ldvt >= NF*vt_stride)",
+              (long long)NF, (long long)L, heads, d, (long long)ldq, (long long)ldk, (long long)ldvt, (long long)ldo, (long long)vt_stride,
+              (long long)nf_nobank);
+    return HV_ERR_INVALID;
+  }
+  const bool bank = Kb != nullptr && Lb > 0;   // a NULL Kb (or Lb = 0) means no bank, whatever the other bank arguments hold
+  if (bank && (!Vbt || F < 1 || NF % F || Lb > INT32_MAX || vbt_stride > INT32_MAX || vbt_stride < Lb || NF / F * Lb > INT32_MAX || NF / F * vbt_stride > INT32_MAX || ldkb < heads * dpad ||
+               (ldkb % 8) || (ldvbt % 8) || ldvbt < NF / F * vbt_stride)) {
+    set_error("hv_op_attention: bad bank arguments NF=%lld F=%lld Lb=%lld ldkb=%lld ldvbt=%lld vbt_stride=%lld (Vbt non-NULL, F divides NF, "
+              "vbt_stride >= Lb, ldkb >= heads*dpad, ldvbt >= (NF/F)*vbt_stride)", (long long)NF, (long long)F, (long long)Lb, (long long)ldkb,
+              (long long)ldvbt, (long long)vbt_stride);
+    return HV_ERR_INVALID;
+  }
+  AttnArgs a;
+  a.q = H(Q); a.k = H(K); a.vt = H(Vt); a.out = HM(out);
+  a.NF = (int)NF; a.L = (int)L; a.heads = heads; a.d = d; a.dpad = (int)dpad;  // V^T rows per head: (d + 1 + 15) / 16 * 16, row d of every head = ones
+  a.ldq = ldq; a.ldk = ldk; a.ldvt = ldvt; a.ldo = ldo;
+  a.kb = H(Kb); a.vbt = H(Vbt); a.Lb = bank ? (int)Lb : 0; a.ldkb = ldkb; a.ldvbt = ldvbt;
+  a.F = (int)F; a.nf_nobank = (int)nf_nobank; a.vt_stride = vt_stride; a.vbt_stride = vbt_stride;
   cudaError_t e = launch_attention(a, device_sms(), ST(stream));
   if (e != cudaSuccess) { set_error("hv_op_attention: %s (%s)", cudaGetErrorString(e), tma_last_error()); return HV_ERR_CUDA; }
   return HV_OK;
@@ -127,7 +147,21 @@ int hv_op_attention_d512(const void* Q, int64_t ldq, const void* K, int64_t ldk,
   return HV_OK;
 }
 
+// rows (b, f, p) and the one-warp-per-problem grid of the register kernel are indexed with ints
+static bool temporal_args_ok(const char* what, int64_t B, int64_t F, int64_t HW, int32_t heads, int32_t d) {
+  const bool d_ok = d == 8 || d == 16 || d == 32 || d == 40 || d == 80 || d == 160;
+  if (B < 1 || B > INT32_MAX || F < 1 || F > 32 || HW < 1 || HW > INT32_MAX || heads < 1 || !d_ok || B * F > INT32_MAX || B * F * HW > INT32_MAX ||
+      B * HW * heads > INT32_MAX || static_cast<int64_t>(heads) * d * 3 > INT32_MAX) {
+    set_error("%s: bad shape B=%lld F=%lld HW=%lld heads=%d d=%d (B, HW, heads >= 1, 1 <= F <= 32, d one of 8, 16, 32, 40, 80, 160)", what,
+              (long long)B, (long long)F, (long long)HW, heads, d);
+    return false;
+  }
+  return true;
+}
+
 int hv_op_temporal_attention(const void* QKV, void* out, int64_t B, int64_t F, int64_t HW, int32_t heads, int32_t d, hv_stream_t stream) {
+  if (!QKV || !out) { set_error("hv_op_temporal_attention: NULL pointer"); return HV_ERR_INVALID; }
+  if (!temporal_args_ok("hv_op_temporal_attention", B, F, HW, heads, d)) return HV_ERR_INVALID;
   CK(launch_temporal_attention(H(QKV), HM(out), (int)B, (int)F, (int)HW, heads, d, ST(stream)), "hv_op_temporal_attention");
 }
 
@@ -196,6 +230,16 @@ int hv_dbg_gemm(const void* A, int64_t lda, const void* W, float* out, int64_t M
 }
 int hv_dbg_gemm_plan(int64_t M, int64_t N, int64_t K, int32_t geglu, int32_t* block_n, int32_t* bst_stages, int32_t* grid) {
   return plan_linear(M, N, K, geglu != 0, block_n, bst_stages, grid);
+}
+int hv_dbg_temporal_attention_plan(int64_t B, int64_t F, int64_t HW, int32_t heads, int32_t d, int32_t* tma, int32_t* heads_per_box, int32_t* grid) {
+  const int sms = device_sms();
+  if (!sms) return HV_ERR_CUDA;
+  if (!temporal_args_ok("hv_dbg_temporal_attention_plan", B, F, HW, heads, d)) return HV_ERR_INVALID;
+  const TemporalPlan p = plan_temporal_attention((int)B, (int)HW, heads, d, sms);
+  if (tma) *tma = p.tma ? 1 : 0;
+  if (heads_per_box) *heads_per_box = p.heads_per_box;
+  if (grid) *grid = (int32_t)p.grid;
+  return HV_OK;
 }
 
 }  // extern "C"

@@ -15,6 +15,15 @@ cudaError_t launch_layernorm(const __half* x, const __half* gamma, const __half*
 cudaError_t launch_clip_embed_ln(const __half* patch, const __half* cls, const __half* pos, const __half* gamma, const __half* beta, __half* out,
                                  long long rows, int L, int C, float eps, cudaStream_t stream);
 cudaError_t launch_temporal_attention(const __half* qkv, __half* out, int B, int F, int HW, int heads, int d, cudaStream_t stream);
+// The kernel launch_temporal_attention runs (one host function decides both the launch and hv_dbg_temporal_attention_plan): the
+// TMA-staged kernel with heads_per_box heads per (pixel, box) and a persistent grid of at most `sms` CTAs, or the register kernel,
+// one warp per (batch item, pixel, head).
+struct TemporalPlan {
+  bool tma;
+  int heads_per_box;
+  unsigned grid;
+};
+TemporalPlan plan_temporal_attention(int B, int HW, int heads, int d, int sms);
 
 struct AttnArgs {
   const __half* q; const __half* k; const __half* vt; __half* out;

@@ -136,7 +136,15 @@ int hv_op_layernorm(const void* X, const void* gamma, const void* beta, void* ou
  * P*V column is the softmax denominator), remaining rows zero; holding
  * V transposed: frame n's tokens occupy columns [n*vt_stride, n*vt_stride + L), vt_stride % 8 == 0.  Optional bank keys/values per batch item (frame n uses bank n / F):
  * Kb [B][Lb][ldkb], Vbt [heads*dv][B*vbt_stride] (same row layout).  Frames with n < nf_nobank attend to their own L keys only (the
- * unconditional CFG half).  out: [NF*L][heads*d].  d is one of 8, 16, 32, 40, 64, 80, 160; other head dims return an error. */
+ * unconditional CFG half).  out: [NF*L][ldo], columns [0, heads*d) written.  d is one of 8, 16, 32, 40, 64, 80, 160; other head dims
+ * return an error.  Kb = NULL or Lb = 0 means no bank (the other bank arguments are then ignored).
+ * A frame's last key tile of 128 is read whole: when L % 128 != 0 the columns [L, vt_stride) of its V^T segment (and the first columns of
+ * the next frame's segment) are loaded and multiplied by P = 0, and likewise [Lb, vbt_stride) of a bank item's segment.  Those columns
+ * must hold finite values (NaN or Inf times 0 is NaN); hv_op_gemm_batched_b writes the pad [rows, round8(rows)) as 0 + rowbias, which
+ * meets this with vt_stride = round8(L).  Columns at or past NF*vt_stride (B*vbt_stride) are never read.
+ * HV_ERR_INVALID unless: the pointers are non-NULL; 1 <= NF <= 65535, 1 <= heads <= 65535, L >= 1, NF*L and NF*vt_stride fit an int32;
+ * 0 <= nf_nobank <= NF; ldo >= heads*d; ldq, ldk >= heads*dpad; ldvt >= NF*vt_stride; vt_stride >= L.  With a bank also: Vbt non-NULL,
+ * F >= 1 divides NF (B = NF/F), vbt_stride >= Lb, ldkb >= heads*dpad, ldvbt >= B*vbt_stride. */
 int hv_op_attention(const void* Q, const void* K, const void* Vt, void* out, int64_t NF, int64_t L, int32_t heads,
                     int32_t d, int64_t ldq, int64_t ldk, int64_t ldvt, int64_t ldo, const void* Kb, const void* Vbt,
                     int64_t Lb, int64_t ldkb, int64_t ldvbt, int64_t F, int64_t nf_nobank, int64_t vt_stride, int64_t vbt_stride,
@@ -150,7 +158,8 @@ int hv_op_attention_d512(const void* Q, int64_t ldq, const void* K, int64_t ldk,
                          int64_t ldo, int64_t NF, int64_t L, hv_stream_t stream);
 
 /* Attention over the frame axis: tokens are rows (b, f, p) of QKV [B*F*HW][3*C] (q | k | v), one problem per
- * (b, p, head) with F <= 32 keys. out [B*F*HW][C]. */
+ * (b, p, head) with F <= 32 keys. out [B*F*HW][C].  HV_ERR_INVALID unless the pointers are non-NULL, B, HW, heads >= 1, 1 <= F <= 32,
+ * d is one of 8, 16, 32, 40, 80, 160 and B*F*HW and B*HW*heads fit an int32. */
 int hv_op_temporal_attention(const void* QKV, void* out, int64_t B, int64_t F, int64_t HW, int32_t heads, int32_t d,
                              hv_stream_t stream);
 
@@ -206,6 +215,10 @@ int hv_dbg_gemm(const void* A, int64_t lda, const void* W, float* out, int64_t M
  * *block_n (128, 160 or 256), *bst_stages > 0 for the B-stationary variant (the CTA's N x K weight panel stays in shared memory and
  * A streams through that many stages) or 0 for the ring variant, and the persistent *grid.  Launches nothing. */
 int hv_dbg_gemm_plan(int64_t M, int64_t N, int64_t K, int32_t geglu, int32_t* block_n, int32_t* bst_stages, int32_t* grid);
+/* The launch hv_op_temporal_attention makes for these arguments on this device (the same host function decides both): *tma = 1 for the
+ * TMA-staged kernel (HW*heads >= 2048 and d = 80, or d = 40 with even heads) with *heads_per_box heads fetched per box and a persistent
+ * *grid of at most one CTA per SM, or *tma = 0 for the register kernel (one warp per problem, *grid blocks of 8).  Launches nothing. */
+int hv_dbg_temporal_attention_plan(int64_t B, int64_t F, int64_t HW, int32_t heads, int32_t d, int32_t* tma, int32_t* heads_per_box, int32_t* grid);
 
 const char* hv_ops_last_error(void);
 int hv_num_sms(void);
