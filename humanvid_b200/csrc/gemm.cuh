@@ -31,7 +31,8 @@ struct GemmEpilogue {
 struct GemmProblem {
   int M = 0, N = 0;                // logical rows / packed columns of D
   int num_k_blocks = 0;            // ceil(K / 64)
-  int bst_stages = 0;              // set by launch_gemm: A-ring depth of the B-stationary variant
+  int stages = 0;                  // set by launch_gemm: ring depth (A + B tiles, or A tiles only in the B-stationary variant)
+  int epi_slabs = 0;               // set by launch_gemm: 128 x 32 staging slabs of the TMA-store epilogue (0: register stores)
   int a_mode = A_LINEAR;
   int k_split = 0;                 // A_LINEAR: k-blocks taken from tensor map a0 (rest from a1); 0 = all from a0
   int cin_blocks = 0;              // conv: 64-channel blocks per tap
@@ -47,9 +48,13 @@ struct GemmProblem {
 
 // How launch_gemm runs a problem.  bst_stages > 0: the B-stationary variant (each CTA keeps its BLOCK_N x K weight panel in shared
 // memory and streams A through a ring of bst_stages tiles; grid is a multiple of the N tiles).  bst_stages == 0: the ring variant
-// (A and B tiles stream together), one persistent CTA per SM, grid = min(tiles, SMs).
+// (A and B tiles stream together, `stages` deep), one persistent CTA per SM, grid = min(tiles, SMs).
+// epi_slabs > 0: the tile leaves through that many 128-row x 32-column shared-memory slabs and TMA stores (the whole tile when
+// they cover it, else in rounds); 0: register stores.
 struct GemmPlan {
   int bst_stages = 0;
+  int stages = 0;
+  int epi_slabs = 0;
   int grid = 0;
 };
 // The plan launch_gemm follows for (p, block_n); false for a block_n or an empty problem it rejects.
@@ -57,9 +62,11 @@ bool plan_gemm(const GemmProblem& p, int block_n, int num_sms, GemmPlan* plan);
 
 // C[M, N] = A[M, K] * B[N, K]^T  (fp16 in, fp32 accumulate in registers, fused epilogue, fp16 out), CTA tile 128 x block_n.
 // a0/a1: TMA maps of the A operand with 128-row boxes (see make_* helpers in tma.h), b: TMA map of the packed weights [N][K].
+// out / res: make_map_tile_* maps of e.out (ldc) and e.residual (ldr) over the written region [0, n_valid) x rows (linear: 2-D,
+// 3x3 conv: 4-D over the output grid); unused by the up-convolution and batched-B paths, and res unused without a residual.
 // block_n must be 128, 160 or 256 (256 required for geglu); 160 = two exact tiles for the 320-wide layers.
-cudaError_t launch_gemm(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const GemmProblem& p,
-                        const GemmEpilogue& e, int block_n, int num_sms, cudaStream_t stream);
+cudaError_t launch_gemm(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const CUtensorMap& out, const CUtensorMap& res,
+                        const GemmProblem& p, const GemmEpilogue& e, int block_n, int num_sms, cudaStream_t stream);
 
 // Picks the (bn, bh, bw) output-tile box of 128 output pixels with the least padding for an NF x H x W output
 // (every box dimension is a power of two <= 128).

@@ -61,6 +61,38 @@ static void fill_epilogue(GemmEpilogue& e, const hv_epilogue* ep, __half* out, i
   }
 }
 
+// The epilogue's TMA stores and residual loads need 16-byte aligned rows: out and residual on 16-byte boundaries, ldr % 8 == 0
+// (ldc is checked with the shape).
+static int check_epilogue_io(const char* op, const void* out, const hv_epilogue* ep) {
+  if (reinterpret_cast<uintptr_t>(out) % 16) {
+    set_error("%s: out %p is not 16-byte aligned", op, out);
+    return HV_ERR_INVALID;
+  }
+  if (ep && ep->residual) {
+    if (reinterpret_cast<uintptr_t>(ep->residual) % 16 || ep->ldr <= 0 || ep->ldr % 8) {
+      set_error("%s: residual %p with ldr=%d: needs a 16-byte aligned pointer and ldr a positive multiple of 8", op, ep->residual,
+                (int)ep->ldr);
+      return HV_ERR_INVALID;
+    }
+  }
+  return HV_OK;
+}
+
+// Output and residual maps of the staged epilogue: [M][n_valid] (linear) or the conv output grid (NF, H, W) x n_valid.
+static int make_epilogue_maps(const char* op, const GemmProblem& p, const GemmEpilogue& e, CUtensorMap* mo, CUtensorMap* mr) {
+  const bool lin = p.a_mode == A_LINEAR;
+  bool ok = lin ? make_map_tile_2d(mo, e.out, p.M, e.n_valid, e.ldc) : make_map_tile_nhwc(mo, e.out, p.NF, p.H, p.W, e.n_valid, e.ldc, p.bn, p.bh, p.bw);
+  if (ok && e.residual)
+    ok = lin ? make_map_tile_2d(mr, e.residual, p.M, e.n_valid, e.ldr) : make_map_tile_nhwc(mr, e.residual, p.NF, p.H, p.W, e.n_valid, e.ldr, p.bn, p.bh, p.bw);
+  else
+    *mr = *mo;
+  if (!ok) {
+    set_error("%s epilogue map: %s", op, tma_last_error());
+    return HV_ERR_TMA;
+  }
+  return HV_OK;
+}
+
 // Tile width: the candidate that pads N the least (N=320 -> 2 x 160, 640 -> 4 x 160, 384 -> 3 x 128, 1280 -> 5 x 256);
 // ties go to the wider tile (fewer A re-reads per output) unless that leaves SMs idle.
 static int pick_block_n(int64_t N, int64_t m_tiles, bool geglu, int sms) {
@@ -126,6 +158,7 @@ int op_gemm(const __half* A, int64_t lda, const __half* A2, int64_t lda2, int64_
     set_error("hv_op_gemm: geglu needs N %% 256 == 0 (N=%lld)", (long long)N);
     return HV_ERR_INVALID;
   }
+  if (int rc = check_epilogue_io("hv_op_gemm", out, ep)) return rc;
   CUtensorMap ma0, ma1, mb;
   const int64_t Ka = split ? K1 : K;
   int bn;
@@ -137,7 +170,9 @@ int op_gemm(const __half* A, int64_t lda, const __half* A2, int64_t lda2, int64_
   if (!make_map_2d(&mb, W, N, K, K, bn)) { set_error("hv_op_gemm W map: %s", tma_last_error()); return HV_ERR_TMA; }
   GemmEpilogue e;
   fill_epilogue(e, ep, out, ldc, N);
-  cudaError_t err = launch_gemm(ma0, ma1, mb, p, e, bn, sms, stream);
+  CUtensorMap mo, mr;
+  if (int rc = make_epilogue_maps("hv_op_gemm", p, e, &mo, &mr)) return rc;
+  cudaError_t err = launch_gemm(ma0, ma1, mb, mo, mr, p, e, bn, sms, stream);
   if (err != cudaSuccess) return cuda_fail(err, "hv_op_gemm launch");
   return HV_OK;
 }
@@ -169,7 +204,7 @@ int op_gemm_batched_b(const __half* A, int64_t lda, const __half* X, int64_t ldx
   e.ldc = static_cast<int>(ldc);
   e.n_valid = static_cast<int>(rows);
   e.rowbias = rowbias;
-  cudaError_t err = launch_gemm(ma, ma, mb, p, e, bn, sms, stream);
+  cudaError_t err = launch_gemm(ma, ma, mb, mb, mb, p, e, bn, sms, stream);
   if (err != cudaSuccess) return cuda_fail(err, "hv_op_gemm_batched_b launch");
   return HV_OK;
 }
@@ -195,6 +230,7 @@ int op_conv3x3(const __half* X, const __half* Wp, __half* out, int64_t ldc, int6
               (long long)Cin, (long long)Cout, stride);
     return HV_ERR_INVALID;
   }
+  if (int rc = check_epilogue_io("hv_op_conv3x3", out, ep)) return rc;
   const int64_t Ho = stride == 1 ? H : H / 2, Wo = stride == 1 ? W : W / 2;
   GemmProblem p;
   p.a_mode = stride == 1 ? A_CONV3X3 : (pad_end ? A_CONV3X3_S2_END : A_CONV3X3_S2);
@@ -210,7 +246,9 @@ int op_conv3x3(const __half* X, const __half* Wp, __half* out, int64_t ldc, int6
   if (!make_map_2d(&mb, Wp, Cout, 9 * Cin, 9 * Cin, bn)) { set_error("hv_op_conv3x3 W map: %s", tma_last_error()); return HV_ERR_TMA; }
   GemmEpilogue e;
   fill_epilogue(e, ep, out, ldc, Cout);
-  cudaError_t err = launch_gemm(ma, ma, mb, p, e, bn, sms, stream);
+  CUtensorMap mo, mr;
+  if (int rc = make_epilogue_maps("hv_op_conv3x3", p, e, &mo, &mr)) return rc;
+  cudaError_t err = launch_gemm(ma, ma, mb, mo, mr, p, e, bn, sms, stream);
   if (err != cudaSuccess) return cuda_fail(err, "hv_op_conv3x3 launch");
   return HV_OK;
 }
@@ -242,7 +280,7 @@ int op_upconv2x2(const __half* X, const __half* Wp, __half* out, int64_t ldc, in
   if (!make_map_2d(&mb, Wp, 4 * Cout, 4 * Cin, 4 * Cin, bn)) { set_error("hv_op_upconv2x2 W map: %s", tma_last_error()); return HV_ERR_TMA; }
   GemmEpilogue e;
   fill_epilogue(e, ep, out, ldc, Cout);
-  cudaError_t err = launch_gemm(ma, ma, mb, p, e, bn, sms, stream);
+  cudaError_t err = launch_gemm(ma, ma, mb, mb, mb, p, e, bn, sms, stream);
   if (err != cudaSuccess) return cuda_fail(err, "hv_op_upconv2x2 launch");
   return HV_OK;
 }

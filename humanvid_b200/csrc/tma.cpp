@@ -95,4 +95,18 @@ bool make_map_nhwc_s2(CUtensorMap* m, const void* ptr, int64_t N, int64_t H, int
   return encode(m, ptr, 5, dims, strides, box);
 }
 
+bool make_map_tile_2d(CUtensorMap* m, const void* ptr, int64_t rows, int64_t cols, int64_t ld) {
+  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
+  cuuint32_t box[2] = {32, 128};
+  return encode(m, ptr, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_64B);
+}
+
+bool make_map_tile_nhwc(CUtensorMap* m, const void* ptr, int64_t N, int64_t H, int64_t W, int64_t cols, int64_t ld, int bn, int bh, int bw) {
+  cuuint64_t dims[4] = {(cuuint64_t)cols, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
+  cuuint64_t strides[3] = {(cuuint64_t)ld * 2, (cuuint64_t)W * ld * 2, (cuuint64_t)H * W * ld * 2};
+  cuuint32_t box[4] = {32, (cuuint32_t)bw, (cuuint32_t)bh, (cuuint32_t)bn};
+  return encode(m, ptr, 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_64B);
+}
+
 }  // namespace hv

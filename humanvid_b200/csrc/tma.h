@@ -35,6 +35,13 @@ bool make_map_col_batches(CUtensorMap* m, const void* ptr, int64_t batch, int64_
 // (box_cols, 1, box_frames) = the box_frames rows of ONE pixel, box_cols channels wide (temporal attention operands).
 bool make_map_frames(CUtensorMap* m, const void* ptr, int64_t frames, int64_t pixels, int64_t cols, int64_t ld, int box_cols, int box_frames);
 
+// GEMM output / residual tiles, 32 columns per box with 64B swizzle (the staging slab of gemm_kernel's epilogue).  Only
+// [0, cols) x rows is inside the map, so a store writes no element outside it and a load reads zero there.
+//   2-D: [rows][ld] -> (cols, rows), box (32, 128)
+//   4-D: channels-last (N, H, W, ld) -> (cols, W, H, N), box (32, bw, bh, bn)
+bool make_map_tile_2d(CUtensorMap* m, const void* ptr, int64_t rows, int64_t cols, int64_t ld);
+bool make_map_tile_nhwc(CUtensorMap* m, const void* ptr, int64_t N, int64_t H, int64_t W, int64_t cols, int64_t ld, int bn, int bh, int bw);
+
 const char* tma_last_error();
 
 }  // namespace hv

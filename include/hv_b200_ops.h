@@ -52,7 +52,7 @@ typedef struct hv_epilogue {
   const void* rowvec;    /* fp16 [groups][rowvec_ld] or NULL (time-embedding projection per batch item) */
   int32_t rowvec_ld;
   int32_t rows_per_group;
-  const void* residual;  /* fp16 [rows][ldr] or NULL */
+  const void* residual;  /* fp16 [rows][ldr] or NULL; 16-byte aligned, ldr > 0 and a multiple of 8 (else HV_ERR_INVALID) */
   int32_t ldr;
   int32_t act;           /* hv_act */
   int32_t geglu;
