@@ -89,6 +89,31 @@ int hv_op_groupnorm(const void* X, int64_t C1, const void* X2, int64_t C2, const
      "hv_op_groupnorm");
 }
 
+size_t hv_groupnorm_pooled_scratch_floats(int64_t C, int64_t NF, int64_t HW, int32_t groups, int64_t frames_per_item) {
+  (void)frames_per_item;   // the per-frame partials dominate; the items' {mean, rstd} fit where the per-frame ones would go
+  return groupnorm_scratch_floats((int)C, (int)NF, (int)HW, groups);
+}
+
+int hv_op_groupnorm_pooled(const void* X, int64_t C1, const void* X2, int64_t C2, const void* gamma, const void* beta, void* out,
+                           int64_t NF, int64_t HW, int32_t groups, float eps, int32_t silu, int64_t frames_per_item, float* stats,
+                           hv_stream_t stream) {
+  if (!device_sms()) return HV_ERR_CUDA;
+  const int64_t F = frames_per_item;
+  auto a16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+  const bool ok = X && gamma && beta && out && stats && (C2 == 0 || X2) && C1 > 0 && C2 >= 0 && C1 + C2 <= 8192 && NF > 0 && HW > 0 &&
+                  HW <= INT32_MAX && F > 0 && NF % F == 0 && NF <= 65535 && a16(X) && (C2 == 0 || a16(X2)) && a16(gamma) && a16(beta) &&
+                  a16(out) && (reinterpret_cast<uintptr_t>(stats) & 7) == 0 && groupnorm_shape_ok((int)C1, (int)C2, (int)HW, groups);
+  if (!ok) {
+    set_error("hv_op_groupnorm_pooled: bad arguments C1=%lld C2=%lld NF=%lld HW=%lld groups=%d frames_per_item=%lld (NF %% F == 0, 16-byte aligned "
+              "tensors, 8-byte aligned stats, a channel layout hv_op_groupnorm supports)", (long long)C1, (long long)C2, (long long)NF, (long long)HW,
+              groups, (long long)F);
+    return HV_ERR_INVALID;
+  }
+  CK(launch_groupnorm_pooled(H(X), (int)C1, C2 ? H(X2) : nullptr, (int)C2, H(gamma), H(beta), HM(out), (int)NF, (int)HW, groups, eps, silu, (int)F,
+                             stats, ST(stream)),
+     "hv_op_groupnorm_pooled");
+}
+
 int hv_op_layernorm(const void* X, const void* gamma, const void* beta, void* out, int64_t rows, int64_t C, float eps,
                     const void* pre_add, int64_t rows_per_group, void* x_out, const void* pe, int64_t hw, int64_t F,
                     hv_stream_t stream) {

@@ -8,6 +8,12 @@ namespace hv {
 cudaError_t launch_groupnorm(const __half* x1, int C1, const __half* x2, int C2, const __half* gamma, const __half* beta,
                              __half* out, int NF, int HW, int groups, float eps, int silu, float* stats, cudaStream_t stream);
 size_t groupnorm_scratch_floats(int C, int NF, int HW, int groups);
+// GroupNorm whose statistics span the F frames of each batch item (frames [b*F, (b+1)*F) are item b); NF % F == 0.  Takes the scratch of
+// groupnorm_scratch_floats(C, NF, HW, groups); at F = 1 it is launch_groupnorm.
+cudaError_t launch_groupnorm_pooled(const __half* x1, int C1, const __half* x2, int C2, const __half* gamma, const __half* beta,
+                                    __half* out, int NF, int HW, int groups, float eps, int silu, int F, float* stats, cudaStream_t stream);
+// The channel / group layouts both GroupNorm launchers accept.
+bool groupnorm_shape_ok(int C1, int C2, int HW, int groups);
 cudaError_t launch_layernorm(const __half* x, const __half* gamma, const __half* beta, __half* out, long long rows, int C, float eps,
                              const __half* pre_add, long long rows_per_group, __half* x_out, const __half* pe, int hw, int F,
                              cudaStream_t stream);

@@ -511,7 +511,7 @@ struct hv_model {
       down.push_back(std::move(s));
       prev = ch[i];
     }
-    mid = stage("mid_block", {ch[3], ch[3]}, ch[3], temb, 1, mm ? 1 : 0);
+    mid = stage("mid_block", {ch[3], ch[3]}, ch[3], temb, 1, (mm && !cfg.no_mid_motion_module) ? 1 : 0);
     const int rev[4] = {ch[3], ch[2], ch[1], ch[0]};
     prev = rev[0];
     for (int i = 0; i < 4; ++i) {
@@ -720,17 +720,28 @@ struct hv_model {
   }
   __half* alloc_h(int64_t n) { return static_cast<__half*>(ar.alloc(static_cast<size_t>(n) * 2)); }
 
-  Tens op_gn(const Tens& x, const Tens* x2, const Norm& n, bool silu) {
+  // pool_F > 1: statistics over the pool_F frames of each batch item (same scratch; one finalize launch more)
+  Tens op_gn(const Tens& x, const Tens* x2, const Norm& n, bool silu, int pool_F = 1) {
     const int C2 = x2 ? x2->C : 0;
     if (n.C != x.C + C2) fail(HV_ERR_INVALID, "groupnorm width %d != %d + %d", n.C, x.C, C2);
     Tens out = alloc_act(x.NF, x.H, x.W, x.C + C2);
     float* stats = static_cast<float*>(ar.alloc(sizeof(float) * groupnorm_scratch_floats(x.C + C2, x.NF, x.H * x.W, cfg.norm_groups)));
+    if (pool_F > 1) {
+      launch(3, {CAT_NORM, "groupnorm_pooled", 0, x.rows(), x.C + C2, 0}, [&] {   // statistics + finalize + apply
+        ck(launch_groupnorm_pooled(x.p, x.C, x2 ? x2->p : nullptr, C2, n.g, n.b, out.p, x.NF, x.H * x.W, cfg.norm_groups, n.eps, silu ? 1 : 0, pool_F,
+                                   stats, st),
+           "groupnorm (pooled over frames)");
+      });
+      return out;
+    }
     launch(2, {CAT_NORM, "groupnorm", 0, x.rows(), x.C + C2, 0}, [&] {   // statistics + apply
       ck(launch_groupnorm(x.p, x.C, x2 ? x2->p : nullptr, C2, n.g, n.b, out.p, x.NF, x.H * x.W, cfg.norm_groups, n.eps, silu ? 1 : 0, stats, st),
          "groupnorm");
     });
     return out;
   }
+  // frames per batch item the resnet / conv_norm_out GroupNorms pool their statistics over (use_inflated_groupnorm=False); 1 = per frame
+  int gn_pool(int F) const { return (cfg.kind == HV_KIND_UNET3D && cfg.gn_pool_frames) ? F : 1; }
   // out = LN(x (+ pre_add per batch item)) (+ pe per frame); returns the normalised tensor, x_new receives x + pre_add
   Tens op_ln(const Tens& x, const Norm& n, const __half* pre_add, int64_t rows_per_b, Tens* x_new, const __half* pe, int F) {
     Tens out = alloc_act(x.NF, x.H, x.W, x.C);
@@ -806,9 +817,9 @@ struct hv_model {
     }
     Scope s(ar);
     __half* tproj = r.has_temb ? op_small_linear(emb, r.temb, B, HV_ACT_SILU) : nullptr;  // time_emb_proj(silu(emb)) : [B][cout]
-    Tens h = op_gn(x, x2, r.n1, true);
+    Tens h = op_gn(x, x2, r.n1, true, gn_pool(F));
     Tens h1 = op_conv3(h, r.c1, 1, tproj, static_cast<int64_t>(F) * x.H * x.W, HV_ACT_NONE, nullptr);
-    Tens h2 = op_gn(h1, nullptr, r.n2, true);
+    Tens h2 = op_gn(h1, nullptr, r.n2, true, gn_pool(F));
     Tens res = x;
     if (r.has_sc) {
       res = alloc_act(x.NF, x.H, x.W, r.cout);
@@ -1043,7 +1054,7 @@ struct hv_model {
       if (outp != nullptr) launch(1, {}, [&] { ck(launch_nhwc_to_ncfhw(h.p, h.C, outp, B, ch[0], F, H, W, st), "hidden layout"); });
       return;
     }
-    Tens hn = op_gn(h, nullptr, norm_out, true);
+    Tens hn = op_gn(h, nullptr, norm_out, true, gn_pool(F));
     Tens y = op_conv3(hn, conv_out, 1, nullptr, 1, HV_ACT_NONE, nullptr);
     launch(1, {}, [&] { ck(launch_nhwc_to_ncfhw(y.p, y.C, outp, B, cfg.out_channels, F, H, W, st), "output layout"); });
   }

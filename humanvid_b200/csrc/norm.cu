@@ -39,11 +39,9 @@ __device__ __forceinline__ float gn_pivot(const __half* __restrict__ x1, int C1,
 }
 
 // grid (slabs, NF); thread = (row lane, 8-channel vector).  Each block writes its per-group {sum, sumsq} of x - pivot to
-// partial[n][slab][g]; gn_apply_kernel adds the slabs in a fixed order -> {mean, rstd}.
-// The launch bounds let ptxas use 56 registers: without them it keeps the kernel at 40 and issues the row loop's four loads one at a
-// time (one 16-byte load in flight per thread; GroupNorm took 27 % longer in a VAE decode).
-__global__ void __launch_bounds__(1024, 1) gn_stats_kernel(const __half* __restrict__ x1, int C1, const __half* __restrict__ x2, int C2, int HW, int groups,
-                                int rows_per_block, float* __restrict__ partial) {
+// partial[n][slab][g]; gn_apply_kernel adds the slabs in a fixed order -> {mean, rstd}.  The pivots are read from frame pn.
+__device__ __forceinline__ void gn_stats_body(const __half* __restrict__ x1, int C1, const __half* __restrict__ x2, int C2, int HW, int groups,
+                                              int rows_per_block, float* __restrict__ partial, int pn) {
   extern __shared__ float sred[];  // [blockDim.x][4][2]
   const int C = C1 + C2, vecs = C / 8, cpg = C / groups;
   const int n = blockIdx.y;
@@ -51,7 +49,7 @@ __global__ void __launch_bounds__(1024, 1) gn_stats_kernel(const __half* __restr
   const int c0 = v * 8;
   float s[4] = {0, 0, 0, 0}, q[4] = {0, 0, 0, 0}, pv[4];
 #pragma unroll
-  for (int i = 0; i < 4; ++i) pv[i] = gn_pivot(x1, C1, x2, C2, HW, n, (c0 + 2 * i) / cpg * cpg);   // a half2 never straddles two groups
+  for (int i = 0; i < 4; ++i) pv[i] = gn_pivot(x1, C1, x2, C2, HW, pn, (c0 + 2 * i) / cpg * cpg);   // a half2 never straddles two groups
   {
     const __half* src;
     int ldc, cc;
@@ -108,6 +106,103 @@ __global__ void __launch_bounds__(1024, 1) gn_stats_kernel(const __half* __restr
     dst[0] = ss;
     dst[1] = qq;
   }
+}
+
+// The launch bounds let ptxas use 56 registers: without them it keeps the kernel at 40 and issues the row loop's four loads one at a
+// time (one 16-byte load in flight per thread; GroupNorm took 27 % longer in a VAE decode).
+__global__ void __launch_bounds__(1024, 1) gn_stats_kernel(const __half* __restrict__ x1, int C1, const __half* __restrict__ x2, int C2, int HW, int groups,
+                                int rows_per_block, float* __restrict__ partial) {
+  gn_stats_body(x1, C1, x2, C2, HW, groups, rows_per_block, partial, blockIdx.y);
+}
+
+// Frame-pooled statistics: the same per-frame partial sums, taken relative to the pivot of the batch item's first frame (frames
+// [b*F, (b+1)*F) are item b), so that the F frames' partials of one (item, group) add up without a per-frame correction.
+__global__ void __launch_bounds__(1024, 1) gn_stats_pooled_kernel(const __half* __restrict__ x1, int C1, const __half* __restrict__ x2, int C2, int HW,
+                                                                  int groups, int rows_per_block, float* __restrict__ partial, int F) {
+  gn_stats_body(x1, C1, x2, C2, HW, groups, rows_per_block, partial, blockIdx.y - blockIdx.y % F);
+}
+
+// grid (groups, items), 128 threads: {mean, rstd} of one (item, group) from the F * slabs partials of its frames.  Thread t adds partials
+// t, t + 128, ... in order, then a fixed tree over the block: the order depends on F * slabs only, never on the number of items.
+constexpr int kGnFinalizeThreads = 128;
+__global__ void __launch_bounds__(kGnFinalizeThreads) gn_finalize_pooled_kernel(const __half* __restrict__ x1, int C1, const __half* __restrict__ x2,
+                                                                                int C2, int HW, int groups, const float* __restrict__ partial,
+                                                                                int slabs, int F, float inv_cnt, float eps, float2* __restrict__ stat) {
+  __shared__ float2 sh[kGnFinalizeThreads / 32];
+  const int g = blockIdx.x, b = blockIdx.y, P = F * slabs;
+  const float* base = partial + (static_cast<long long>(b) * P * groups + g) * 2;   // partial[b*F + f][slab][g] = base[(f * slabs + slab) * groups * 2]
+  float ss = 0.f, qq = 0.f;
+  for (int p = threadIdx.x; p < P; p += kGnFinalizeThreads) {
+    const float2 pp = __ldg(reinterpret_cast<const float2*>(base + static_cast<long long>(p) * groups * 2));
+    ss += pp.x;
+    qq += pp.y;
+  }
+#pragma unroll
+  for (int o = 16; o; o >>= 1) {
+    ss += __shfl_xor_sync(0xffffffffu, ss, o);
+    qq += __shfl_xor_sync(0xffffffffu, qq, o);
+  }
+  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = make_float2(ss, qq);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    ss = (sh[0].x + sh[1].x) + (sh[2].x + sh[3].x);
+    qq = (sh[0].y + sh[1].y) + (sh[2].y + sh[3].y);
+    const float m = ss * inv_cnt;   // mean - pivot
+    const int cpg = (C1 + C2) / groups;
+    stat[static_cast<long long>(b) * groups + g] =
+        make_float2(gn_pivot(x1, C1, x2, C2, HW, b * F, g * cpg) + m, rsqrtf(fmaxf(qq * inv_cnt - m * m, 0.f) + eps));
+  }
+}
+
+// Normalises rows [blockIdx.x * rows_per_block, ...) of frame blockIdx.y with the per-group {mean, rstd} in sstat.  (gn_apply_kernel keeps
+// its own copy of this loop: calling this function from it reorders its SASS.)
+__device__ __forceinline__ void gn_apply_rows(const __half* __restrict__ x1, int C1, const __half* __restrict__ x2, int C2,
+                                              const __half* __restrict__ gamma, const __half* __restrict__ beta, __half* __restrict__ out,
+                                              int HW, int groups, int rows_per_block, int silu, const float2* sstat) {
+  const int C = C1 + C2, vecs = C / 8, cpg = C / groups;
+  const int n = blockIdx.y;
+  const int rl = threadIdx.x / vecs, v = threadIdx.x % vecs, rpi = blockDim.x / vecs;
+  const int c0 = v * 8;
+  float sc[8], sh[8];
+  {
+    float gm[8], bt[8];
+    unpack8(__ldg(reinterpret_cast<const uint4*>(gamma + c0)), gm);
+    unpack8(__ldg(reinterpret_cast<const uint4*>(beta + c0)), bt);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const float2 st = sstat[(c0 + 2 * k) / cpg];
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        sc[2 * k + j] = st.y * gm[2 * k + j];
+        sh[2 * k + j] = fmaf(-st.x, sc[2 * k + j], bt[2 * k + j]);
+      }
+    }
+  }
+  const __half* src;
+  int ldc;
+  if (c0 < C1) { src = x1 + static_cast<long long>(n) * HW * C1 + c0; ldc = C1; } else { src = x2 + static_cast<long long>(n) * HW * C2 + (c0 - C1); ldc = C2; }
+  __half* dst = out + static_cast<long long>(n) * HW * C + c0;
+  const int row_end = min(HW, (blockIdx.x + 1) * rows_per_block);
+  auto emit = [&](const uint4& u, int r) {
+    float f[8];
+    unpack8(u, f);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      float y = fmaf(f[j], sc[j], sh[j]);
+      if (silu) y = __fdividef(y, 1.0f + __expf(-y));
+      f[j] = y;
+    }
+    *reinterpret_cast<uint4*>(dst + static_cast<long long>(r) * C) = pack8(f);
+  };
+  int r = blockIdx.x * rows_per_block + rl;
+  for (; r + 3 * rpi < row_end; r += 4 * rpi) {
+    uint4 u[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) u[k] = __ldg(reinterpret_cast<const uint4*>(src + static_cast<long long>(r + k * rpi) * ldc));
+#pragma unroll
+    for (int k = 0; k < 4; ++k) emit(u[k], r + k * rpi);
+  }
+  for (; r < row_end; r += rpi) emit(__ldg(reinterpret_cast<const uint4*>(src + static_cast<long long>(r) * ldc)), r);
 }
 
 // grid (slabs, NF), thread = (row lane, 8-channel vector) like the statistics kernel: the thread's channels are fixed, so
@@ -188,6 +283,13 @@ __global__ void gn_apply_kernel(const __half* __restrict__ x1, int C1, const __h
     for (int k = 0; k < 4; ++k) emit(u[k], r + k * rpi);
   }
   for (; r < row_end; r += rpi) emit(__ldg(reinterpret_cast<const uint4*>(src + static_cast<long long>(r) * ldc)), r);
+}
+
+// Frame-pooled apply: frame n of item n / F reads the item's {mean, rstd} written by gn_finalize_pooled_kernel.
+__global__ void gn_apply_pooled_kernel(const __half* __restrict__ x1, int C1, const __half* __restrict__ x2, int C2,
+                                       const __half* __restrict__ gamma, const __half* __restrict__ beta, __half* __restrict__ out,
+                                       int HW, int groups, int rows_per_block, int silu, const float2* __restrict__ stat, int F) {
+  gn_apply_rows(x1, C1, x2, C2, gamma, beta, out, HW, groups, rows_per_block, silu, stat + static_cast<long long>(blockIdx.y / F) * groups);
 }
 
 // ---------------------------------------------------------------- LayerNorm: one warp per row
@@ -369,20 +471,47 @@ size_t groupnorm_scratch_floats(int C, int NF, int HW, int groups) {
   return static_cast<size_t>(2) * NF * groups * (1 + sl);
 }
 
+bool groupnorm_shape_ok(int C1, int C2, int HW, int groups) {
+  const int C = C1 + C2;
+  if (groups <= 0 || C % 8 || C1 % 8 || C % groups || ((C / groups) & 1) || groups > 32 * 8) return false;
+  const int vecs = C / 8;
+  if (vecs > 1024) return false;
+  int threads, slabs, rows_per_block;
+  gn_plan(C, HW, &threads, &slabs, &rows_per_block);
+  return threads >= groups && threads >= 32;
+}
+
 cudaError_t launch_groupnorm(const __half* x1, int C1, const __half* x2, int C2, const __half* gamma, const __half* beta,
                              __half* out, int NF, int HW, int groups, float eps, int silu, float* stats, cudaStream_t stream) {
   const int C = C1 + C2;
-  if (C % 8 || C1 % 8 || C % groups || ((C / groups) & 1) || groups > 32 * 8) return cudaErrorInvalidValue;
-  const int vecs = C / 8;
-  if (vecs > 1024) return cudaErrorInvalidValue;
+  if (!groupnorm_shape_ok(C1, C2, HW, groups)) return cudaErrorInvalidValue;
   int threads, slabs, rows_per_block;
   gn_plan(C, HW, &threads, &slabs, &rows_per_block);
-  if (threads < groups || threads < 32) return cudaErrorInvalidValue;
   float* partial = stats + static_cast<size_t>(2) * NF * groups;
   gn_stats_kernel<<<dim3(slabs, NF), threads, threads * 8 * sizeof(float), stream>>>(x1, C1, x2, C2, HW, groups, rows_per_block, partial);
   // (the {mean, rstd} finalize is folded into the apply kernel: one launch less per GroupNorm, 83 per forward)
   gn_apply_kernel<<<dim3(slabs, NF), threads, groups * sizeof(float2), stream>>>(x1, C1, x2, C2, gamma, beta, out, HW, groups, rows_per_block, silu, partial,
                                                                                  slabs, 1.f / (static_cast<float>(HW) * (C / groups)), eps);
+  return cudaGetLastError();
+}
+
+// Statistics pooled over the F frames of each batch item (nn.GroupNorm on a (b, c, f, h, w) tensor).  Same scratch as launch_groupnorm:
+// the per-frame partials at the same offset, and the items' {mean, rstd} in the first 2 * (NF / F) * groups floats.  At F = 1 this is
+// launch_groupnorm itself.
+cudaError_t launch_groupnorm_pooled(const __half* x1, int C1, const __half* x2, int C2, const __half* gamma, const __half* beta,
+                                    __half* out, int NF, int HW, int groups, float eps, int silu, int F, float* stats, cudaStream_t stream) {
+  if (F <= 0 || NF % F) return cudaErrorInvalidValue;
+  if (F == 1) return launch_groupnorm(x1, C1, x2, C2, gamma, beta, out, NF, HW, groups, eps, silu, stats, stream);
+  const int C = C1 + C2;
+  if (!groupnorm_shape_ok(C1, C2, HW, groups)) return cudaErrorInvalidValue;
+  int threads, slabs, rows_per_block;
+  gn_plan(C, HW, &threads, &slabs, &rows_per_block);
+  float2* stat = reinterpret_cast<float2*>(stats);
+  float* partial = stats + static_cast<size_t>(2) * NF * groups;
+  gn_stats_pooled_kernel<<<dim3(slabs, NF), threads, threads * 8 * sizeof(float), stream>>>(x1, C1, x2, C2, HW, groups, rows_per_block, partial, F);
+  gn_finalize_pooled_kernel<<<dim3(groups, NF / F), kGnFinalizeThreads, 0, stream>>>(x1, C1, x2, C2, HW, groups, partial, slabs, F,
+                                                                                      1.f / (static_cast<float>(F) * HW * (C / groups)), eps, stat);
+  gn_apply_pooled_kernel<<<dim3(slabs, NF), threads, 0, stream>>>(x1, C1, x2, C2, gamma, beta, out, HW, groups, rows_per_block, silu, stat, F);
   return cudaGetLastError();
 }
 

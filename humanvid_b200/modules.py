@@ -275,9 +275,10 @@ class _NativeNet(nn.Module):
         self._bank_refs = None
         self._reserved = set()
 
-    def _reserve(self, h, B, F, H, W):
-        """The C forwards never allocate: grow the handle's private workspace here, once per new shape."""
-        key = (B, F, H, W)
+    def _reserve(self, h, B, F, H, W, variant=()):
+        """The C forwards never allocate: grow the handle's private workspace here, once per new shape (and `variant`: whatever
+        else the plan depends on, such as the reference banks of the denoising UNet)."""
+        key = (B, F, H, W, variant)
         if key not in self._reserved:
             N.check(N.lib().hv_reserve_workspace(h, N.i32(B), N.i32(F), N.i32(H), N.i32(W)), h)
             self._reserved.add(key)
@@ -360,6 +361,8 @@ class HvConfig(C.Structure):
         ("clip_image_size", C.c_int32),
         ("clip_projection_dim", C.c_int32),
         ("clip_layer_norm_eps", C.c_float),
+        ("gn_pool_frames", C.c_int32),
+        ("no_mid_motion_module", C.c_int32),
     ]
 
 
@@ -420,14 +423,15 @@ class UNet3DConditionModel(_NativeNet):
         if resnet_time_scale_shift != "default" or act_fn not in ("silu", "swish") or mid_block_scale_factor != 1 or not isinstance(attention_head_dim, int):
             unsupported.append("non-default resnet/act options")
         if use_motion_module and (
-            tuple(motion_module_resolutions) != (1, 2, 4, 8) or not motion_module_mid_block or motion_module_decoder_only
+            tuple(motion_module_resolutions) != (1, 2, 4, 8) or motion_module_decoder_only
             or motion_module_type != "Vanilla" or mmk.get("num_transformer_block", 1) != 1
             or tuple(mmk.get("attention_block_types", ("Temporal_Self", "Temporal_Self"))) != ("Temporal_Self", "Temporal_Self")
             or not mmk.get("temporal_position_encoding", False) or mmk.get("temporal_attention_dim_div", 1) != 1
         ):
-            unsupported.append("motion-module layout other than configs/inference/inference_v2.yaml")
+            unsupported.append("motion-module layout other than configs/inference/inference_v1.yaml / inference_v2.yaml")
         if unsupported:
-            raise NotImplementedError("humanvid_b200.UNet3DConditionModel implements the inference_v2 hot path only; unsupported: " + "; ".join(unsupported))
+            raise NotImplementedError("humanvid_b200.UNet3DConditionModel implements the inference_v1 / inference_v2 hot path only; unsupported: "
+                                      + "; ".join(unsupported))
         self.config = SimpleNamespace(**{k: v for k, v in locals().items() if k not in ("self", "mmk", "unsupported", "__class__")})
         self.sample_size = sample_size
         self.in_channels = in_channels
@@ -437,6 +441,7 @@ class UNet3DConditionModel(_NativeNet):
         mm = bool(use_motion_module)
         max_len = mmk.get("temporal_position_encoding_max_len", 24)
         self._heads, self._max_len, self._mm = heads, max_len, mm
+        mid_mm = mm and bool(motion_module_mid_block)   # inference_v1.yaml: no motion module in the mid block
         self.conv_in = _conv(in_channels, ch[0], 3, padding=1)
         self.time_embedding = _TimestepEmbedding(ch[0], temb)
         self.down_blocks = nn.ModuleList([])
@@ -447,7 +452,7 @@ class UNet3DConditionModel(_NativeNet):
             last = i == 3
             self.down_blocks.append(_Block([(prev, c), (c, c)], c, 0 if last else 2, mm, xdim, temb, g, max_len, None if last else "down"))
             prev = c
-        self.mid_block = _Block([(ch[3], ch[3]), (ch[3], ch[3])], ch[3], 1, mm, xdim, temb, g, max_len, "mid")
+        self.mid_block = _Block([(ch[3], ch[3]), (ch[3], ch[3])], ch[3], 1, mid_mm, xdim, temb, g, max_len, "mid")
         rev = ch[::-1]
         prev = rev[0]
         for i, c in enumerate(rev):
@@ -517,6 +522,9 @@ class UNet3DConditionModel(_NativeNet):
         cfg.block_out_channels = (C.c_int32 * 4)(*c.block_out_channels)
         cfg.heads, cfg.cross_attention_dim, cfg.norm_groups = c.attention_head_dim, c.cross_attention_dim, c.norm_num_groups
         cfg.use_motion_module, cfg.motion_max_len = int(self._mm), self._max_len
+        # use_inflated_groupnorm=False: the resnets and conv_norm_out apply nn.GroupNorm to (b, c, f, h, w), pooling over the frames
+        cfg.gn_pool_frames = int(not c.use_inflated_groupnorm)
+        cfg.no_mid_motion_module = int(self._mm and not c.motion_module_mid_block)
         return cfg
 
     # ---- debug taps (per-layer error ladder; scripts/error_ladder.py) ---------------------------------------------------
@@ -568,11 +576,6 @@ class UNet3DConditionModel(_NativeNet):
         B, Cc, F, H, W = sample.shape
         if Cc != self.in_channels:
             raise ValueError(f"sample has {Cc} channels, model expects {self.in_channels}")
-        if F > 1 and not self.config.use_inflated_groupnorm:
-            # resnet.py:158-161: with use_inflated_groupnorm=False the reference applies nn.GroupNorm to the 5-D tensor, pooling the
-            # statistics over frames; the native path normalises per frame (InflatedGroupNorm), identical only when F == 1
-            raise NotImplementedError("use_inflated_groupnorm=False with more than one frame (cross-frame GroupNorm statistics) is not implemented; "
-                                      "the inference_v2 configuration sets use_inflated_groupnorm=True")
         h = self._sync_native()
         self._push_banks(h)
         x = self._as_half(sample, "sample")
@@ -585,7 +588,7 @@ class UNet3DConditionModel(_NativeNet):
         t = int(timestep.reshape(-1)[0].item()) if torch.is_tensor(timestep) else int(timestep)
         out = torch.empty((B, self.config.out_channels, F, H, W), device=x.device, dtype=torch.float16)
         flags = self._forward_flags if self._forward_flags is not None else (1 if self._ref_cfg else 0)
-        self._reserve(h, B, F, H, W)
+        self._reserve(h, B, F, H, W, tuple(tuple(t.shape) for t in (self._bank_refs or ())))   # the banks' K/V scratch is planned too
         N.check(N.lib().hv_unet3d_forward(h, N.ptr(x), N.i64(t), N.ptr(ehs), N.ptr(pose), N.ptr(out), N.i32(B), N.i32(F), N.i32(H), N.i32(W),
                                           C.c_uint32(flags), None, C.c_size_t(0), N.stream()), h)
         out = out.to(sample.dtype) if sample.dtype != torch.float16 else out

@@ -80,6 +80,11 @@ typedef struct hv_config {
   int32_t clip_image_size;        /* 224 */
   int32_t clip_projection_dim;    /* 768 */
   float clip_layer_norm_eps;      /* 1e-5 */
+  /* UNet3DConditionModel, configs/inference/inference_v1.yaml (AnimateDiff v1 motion-module layout).  0 keeps the inference_v2 behaviour. */
+  int32_t gn_pool_frames;         /* 1: use_inflated_groupnorm = False -- the resnets' norm1 / norm2 and conv_norm_out take their statistics over
+                                     all F frames of a batch item (nn.GroupNorm on (b, c, f, h, w)); the transformer and motion-module
+                                     GroupNorms stay per frame.  A frame's output then depends on the other frames of its window. */
+  int32_t no_mid_motion_module;   /* 1: motion_module_mid_block = False -- the mid block has no motion module */
 } hv_config;
 
 int hv_create(const hv_config* cfg, hv_handle* out);

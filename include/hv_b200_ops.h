@@ -123,6 +123,18 @@ int hv_op_conv3x3_direct(const void* X, const void* W, const void* bias, void* o
 size_t hv_groupnorm_scratch_floats(int64_t C, int64_t NF, int64_t HW, int32_t groups);
 int hv_op_groupnorm(const void* X, int64_t C1, const void* X2, int64_t C2, const void* gamma, const void* beta, void* out,
                     int64_t NF, int64_t HW, int32_t groups, float eps, int32_t silu, float* stats, hv_stream_t stream);
+/* GroupNorm whose statistics span every frame of a batch item: nn.GroupNorm on a (b, c, f, h, w) tensor (unet_3d.py:235-246 and
+ * resnet.py:153-190 with use_inflated_groupnorm=False).  Same layout and options as hv_op_groupnorm; frames [b*F, (b+1)*F) of the
+ * (NF, HW, C1+C2) input are item b, F = frames_per_item.  One pivot per (item, group): the group's first channel in the first row of the
+ * item's first frame.  The summation order depends on (F, HW, C) only, never on NF / F, so an item's output does not depend on the other
+ * items in the call.  At F = 1 this is hv_op_groupnorm, bit for bit.  stats: hv_groupnorm_pooled_scratch_floats(...) fp32.
+ * Returns HV_ERR_INVALID and writes nothing for: NULL pointers (X2 may be NULL only when C2 == 0), NF, HW or F <= 0, NF % F != 0,
+ * NF > 65535, X / X2 / gamma / beta / out not 16-byte aligned or stats not 8-byte aligned, and the channel layouts hv_op_groupnorm cannot
+ * run (C1 + C2 and C1 multiples of 8, C1 + C2 <= 8192, C / groups even, groups <= 256 and <= the block's thread count). */
+size_t hv_groupnorm_pooled_scratch_floats(int64_t C, int64_t NF, int64_t HW, int32_t groups, int64_t frames_per_item);
+int hv_op_groupnorm_pooled(const void* X, int64_t C1, const void* X2, int64_t C2, const void* gamma, const void* beta, void* out,
+                           int64_t NF, int64_t HW, int32_t groups, float eps, int32_t silu, int64_t frames_per_item, float* stats,
+                           hv_stream_t stream);
 
 /* LayerNorm over C per row.  Optional: `pre_add` fp16 [rows / rows_per_group][C] is added to x first and the sum is
  * written to `x_out` (the cross-attention residual, see DESIGN.md); `pe` fp16 [F][C] is added to the normalised row
