@@ -25,7 +25,6 @@ struct GemmEpilogue {
   int act = ACT_NONE;
   int geglu = 0;                   // BLOCK_N=256 tile = [128 hidden | 128 gate] -> 128 outputs
   const __half* rowbias = nullptr; // [M]: added to every column of output row m (the "ones" rows of V^T)
-  float* gn_stats = nullptr;       // reserved (fused GroupNorm statistics)
 };
 
 struct GemmProblem {

@@ -68,6 +68,7 @@ struct Norm {
 struct Lin {
   Mat w;
   __half* bias = nullptr;
+  bool geglu = false;  // packed by ff1_geglu: runs with the GEGLU epilogue, w.rows / 2 outputs
 };
 struct Conv3 {       // implicit-GEMM packed 3x3 conv
   Mat w;             // [cout_pad][9 * cin_pad]
@@ -96,18 +97,22 @@ struct ResnetW {
   Lin sc;
   int cin = 0, cout = 0;
 };
+// Self-attention in the layouts of the attention kernels.  dv > d: the spatial kernel, V^T has a ones row per head (h * dv + d, the
+// softmax denominator) and zero rows up to dv; dv == d: the single-head d = 512 kernel, no ones row.
+struct SelfAttnW {
+  Lin qk;                   // [2 * heads * dpad][C] (+ bias): q rows then k rows, each head zero-padded to dpad
+  Mat wv;                   // [heads * dv][C]: to_v rows of head h at h * dv, zero rows elsewhere
+  __half* vbias = nullptr;  // [heads * dv] row bias of V^T: the ones rows plus to_v's bias at h * dv + j (null when neither exists)
+  Lin out;
+  int heads = 0, d = 0, dpad = 0, dv = 0;
+};
 struct SpatialW {
   Norm gn, ln1, ln3;
   Lin proj_in, proj_out;
-  Mat wqk;   // [2*heads*dpad][C]  (q rows then k rows, each head zero-padded to dpad)
-  Mat wk;    // [heads*dpad][C]    view into wqk (bank keys)
-  Mat wv;    // [heads*dv][C]: to_v rows of head h at h*dv.., zero rows elsewhere (dv = (d+1) rounded up to 16)
-  __half* vones = nullptr;  // [heads*dv]: 1 at row h*dv + d (the softmax-denominator row of V^T), else 0
-  int dv = 0;
-  Lin out1;
+  SelfAttnW attn1;
   Lin v2, out2;  // cross-attention collapse: to_v (C x xdim), to_out
   Lin ff1, ff2;  // ff1 geglu-packed
-  int C = 0, heads = 0, d = 0, dpad = 0;
+  int C = 0;
   int reader_idx = -1;
   // reference bank (B_ref, L, C): `bank` is non-null while a bank is set; its storage (bank_store, bank_cap elements) is kept
   // across hv_clear_ref_banks so that the per-forward clear / set of the Python reader costs no allocation
@@ -119,36 +124,30 @@ struct SpatialW {
 };
 struct TAttnW {
   Norm ln;
-  Mat wqkv;  // [3C][C]
+  Lin qkv;   // [3C][C], no bias
   Lin out;
   __half* pe = nullptr;  // [max_len][C]
   int max_len = 0;
 };
-struct MotionW {
-  Norm gn, ffn;
-  Lin proj_in, proj_out, ff1, ff2;
+struct TBlockW {   // TemporalTransformerBlock: temporal self-attentions, then LayerNorm -> GEGLU feed-forward + residual
   std::vector<TAttnW> attn;
-  int C = 0, heads = 0, d = 0;
+  Norm ff_norm;
+  Lin ff1, ff2;      // ff1 geglu-packed
+  int heads = 0, d = 0;
+};
+struct MotionW {
+  Norm gn;
+  Lin proj_in, proj_out;
+  TBlockW block;
 };
 struct CamResW {
   Conv3 block1;
   Lin block2;
 };
-struct VaeAttnW {   // AutoencoderKL mid-block attention: one head of C = 512 channels, biased q / k / v
-  Norm gn;
-  Mat wqk;          // [2C][C]: to_q rows then to_k rows
-  __half* bqk = nullptr;
-  Mat wv;           // [C][C] (the "A" operand of the V^T GEMM)
-  __half* bv = nullptr;
-  Lin out;
-};
 struct ClipLayerW {   // CLIPEncoderLayer: pre-LN self-attention (heads of d = 64, biased q / k / v) and a quick-GELU MLP
   Norm ln1, ln2;
-  Mat wqk;            // [2 * hidden][hidden]: q_proj rows then k_proj rows (d = 64 needs no head padding)
-  __half* bqk = nullptr;
-  Mat wv;             // [heads * dv][hidden]: v_proj rows of head h at h * dv, zero rows elsewhere (dv = 80)
-  __half* bv = nullptr;  // [heads * dv]: v_proj's bias at h * dv + j, 1 at h * dv + 64 (the softmax-denominator row of V^T), else 0
-  Lin out, fc1, fc2;
+  SelfAttnW attn;
+  Lin fc1, fc2;
 };
 
 // ------------------------------------------------------------------------------------------ workspace arena
@@ -264,14 +263,15 @@ struct hv_model {
   // ---- CameraPoseEncoder
   Conv3 cam_in;
   std::vector<CamResW> cam_res;
-  std::vector<MotionW> cam_att;  // reuse MotionW: attn[0] + ff (no gn / proj)
+  std::vector<TBlockW> cam_att;
   Lin cam_zero;
   // ---- AutoencoderKL: encoder.* / decoder.* (the down / up blocks and the mid block's two resnets are Stages without attention)
   struct VaeHalf {
     Conv3 conv_in;
     std::vector<Stage> blocks;
     Stage mid;
-    VaeAttnW attn;
+    Norm attn_gn;    // the mid-block attention: GroupNorm, then one head of C = 512 channels with biased q / k / v
+    SelfAttnW attn;
     Norm norm_out;
     Conv3 conv_out;
   };
@@ -285,7 +285,6 @@ struct hv_model {
   Norm clip_pre, clip_post;
   std::vector<ClipLayerW> clip_layers;
   Mat clip_proj;           // visual_projection [projection_dim][hidden]
-  int clip_dv = 0;
 
   ~hv_model() {
     for (void* p : owned) cudaFree(p);
@@ -391,6 +390,7 @@ struct hv_model {
     ck(launch_pack_geglu(w.p, l.w.p, 8 * C, C, sms, st), "pack geglu");
     l.bias = dmalloc(8LL * C);
     ck(launch_pack_geglu(b.p, l.bias, 8 * C, 1, sms, st), "pack geglu bias");
+    l.geglu = true;
     return l;
   }
 
@@ -418,30 +418,47 @@ struct hv_model {
     ck(cudaStreamSynchronize(st), "vones sync");  // `ones` is a host temporary
     return p;
   }
+  // The projections `keys` ([heads * d][cols] each; cols = 1 for biases) stacked into one matrix: head h of keys[i] at rows
+  // (i * heads + h) * dpad .., zero rows from d to dpad
+  __half* stack_heads(const std::vector<std::string>& keys, int heads, int d, int dpad, int cols) {
+    const int64_t rows = static_cast<int64_t>(heads) * dpad;
+    __half* p = dmalloc(static_cast<int64_t>(keys.size()) * rows * cols);
+    for (size_t i = 0; i < keys.size(); ++i)
+      ck(launch_pack_heads(mat(keys[i], static_cast<int64_t>(heads) * d, cols).p, p + i * rows * cols, heads, d, dpad, cols, sms, st), "pack heads");
+    return p;
+  }
+  // q / k / v / out: key prefixes of the projections; bias: q, k and v have biases (out always has one)
+  SelfAttnW self_attn(const std::string& q, const std::string& k, const std::string& v, const std::string& out, int C, int heads, bool bias) {
+    SelfAttnW a;
+    a.heads = heads;
+    a.d = C / heads;
+    a.dpad = static_cast<int>(rup(a.d, 16));
+    a.dv = (a.d == 512 && heads == 1) ? a.d : static_cast<int>(rup(a.d + 1, 16));
+    a.qk.w = Mat{stack_heads({q + ".weight", k + ".weight"}, heads, a.d, a.dpad, C), 2LL * heads * a.dpad, C};
+    if (bias) a.qk.bias = stack_heads({q + ".bias", k + ".bias"}, heads, a.d, a.dpad, 1);
+    a.wv = Mat{stack_heads({v + ".weight"}, heads, a.d, a.dv, C), static_cast<int64_t>(heads) * a.dv, C};
+    if (a.dv > a.d) a.vbias = vones(heads, a.dv, a.d);
+    else if (bias) a.vbias = dmalloc(static_cast<int64_t>(heads) * a.dv);
+    if (bias)
+      ck(cudaMemcpy2DAsync(a.vbias, static_cast<size_t>(a.dv) * 2, vec(v + ".bias", C), static_cast<size_t>(a.d) * 2, static_cast<size_t>(a.d) * 2, heads,
+                           cudaMemcpyDeviceToDevice, st), "v bias pack");
+    a.out = lin(out, C, C);
+    return a;
+  }
   SpatialW spatial(const std::string& pfx, int C) {
     SpatialW s;
     s.name = pfx;
     s.C = C;
-    s.heads = cfg.heads;
-    s.d = C / cfg.heads;
-    s.dpad = static_cast<int>(rup(s.d, 16));
-    if (s.d % 8) fail(HV_ERR_INVALID, "head dim %d (C=%d / %d heads) must be a multiple of 8", s.d, C, cfg.heads);
+    const int d = C / cfg.heads;
+    if (d % 8) fail(HV_ERR_INVALID, "head dim %d (C=%d / %d heads) must be a multiple of 8", d, C, cfg.heads);
     s.gn = norm(pfx + ".norm", C, 1e-6f);
     s.proj_in = lin(pfx + ".proj_in", C, C);
     s.proj_out = lin(pfx + ".proj_out", C, C);
     const std::string b = pfx + ".transformer_blocks.0";
     s.ln1 = norm(b + ".norm1", C, 1e-5f);
     s.ln3 = norm(b + ".norm3", C, 1e-5f);
-    const int64_t hp = static_cast<int64_t>(s.heads) * s.dpad;
-    s.wqk = Mat{dmalloc(2 * hp * C), 2 * hp, C};
-    ck(launch_pack_heads(mat(b + ".attn1.to_q.weight", C, C).p, s.wqk.p, s.heads, s.d, s.dpad, C, sms, st), "pack q");
-    ck(launch_pack_heads(mat(b + ".attn1.to_k.weight", C, C).p, s.wqk.p + hp * C, s.heads, s.d, s.dpad, C, sms, st), "pack k");
-    s.wk = Mat{s.wqk.p + hp * C, hp, C};
-    s.dv = static_cast<int>(rup(s.d + 1, 16));
-    s.wv = Mat{dmalloc(static_cast<int64_t>(s.heads) * s.dv * C), static_cast<int64_t>(s.heads) * s.dv, C};
-    ck(launch_pack_heads(mat(b + ".attn1.to_v.weight", C, C).p, s.wv.p, s.heads, s.d, s.dv, C, sms, st), "pack v");
-    s.vones = vones(s.heads, s.dv, s.d);
-    s.out1 = lin(b + ".attn1.to_out.0", C, C);
+    const std::string a = b + ".attn1";
+    s.attn1 = self_attn(a + ".to_q", a + ".to_k", a + ".to_v", a + ".to_out.0", C, cfg.heads, false);
     s.v2 = lin(b + ".attn2.to_v", C, cfg.cross_attention_dim, false);
     s.out2 = lin(b + ".attn2.to_out.0", C, C);
     s.ff1 = ff1_geglu(b + ".ff.net.0.proj", C);
@@ -451,11 +468,7 @@ struct hv_model {
   TAttnW tattn(const std::string& attn_pfx, const std::string& norm_pfx, int C) {
     TAttnW t;
     t.ln = norm(norm_pfx, C, 1e-5f);
-    t.wqkv = Mat{dmalloc(3LL * C * C), 3LL * C, C};
-    const char* names[3] = {".to_q.weight", ".to_k.weight", ".to_v.weight"};
-    for (int i = 0; i < 3; ++i)
-      ck(cudaMemcpyAsync(t.wqkv.p + static_cast<int64_t>(i) * C * C, mat(attn_pfx + names[i], C, C).p, static_cast<size_t>(C) * C * 2,
-                         cudaMemcpyDeviceToDevice, st), "qkv concat");
+    t.qkv.w = Mat{stack_heads({attn_pfx + ".to_q.weight", attn_pfx + ".to_k.weight", attn_pfx + ".to_v.weight"}, 1, C, C, C), 3LL * C, C};
     t.out = lin(attn_pfx + ".to_out.0", C, C);
     const Raw& pe = get(attn_pfx + ".pos_encoder.pe");
     if (pe.numel() % C) fail(HV_ERR_INVALID, "'%s.pos_encoder.pe' width != %d", attn_pfx.c_str(), C);
@@ -463,31 +476,35 @@ struct hv_model {
     t.max_len = static_cast<int>(pe.numel() / C);
     return t;
   }
+  // TemporalTransformerBlock `pfx` with n_attn temporal self-attentions
+  TBlockW tblock(const std::string& pfx, int C, int heads, int n_attn) {
+    TBlockW b;
+    b.heads = heads;
+    b.d = C / heads;
+    for (int i = 0; i < n_attn; ++i)
+      b.attn.push_back(tattn(pfx + ".attention_blocks." + std::to_string(i), pfx + ".norms." + std::to_string(i), C));
+    b.ff_norm = norm(pfx + ".ff_norm", C, 1e-5f);
+    b.ff1 = ff1_geglu(pfx + ".ff.net.0.proj", C);
+    b.ff2 = lin(pfx + ".ff.net.2", C, 4 * C);
+    return b;
+  }
   MotionW motion(const std::string& pfx, int C) {
     MotionW m;
-    m.C = C;
-    m.heads = cfg.heads;
-    m.d = C / cfg.heads;
     const std::string t = pfx + ".temporal_transformer";
     m.gn = norm(t + ".norm", C, 1e-6f);
     m.proj_in = lin(t + ".proj_in", C, C);
     m.proj_out = lin(t + ".proj_out", C, C);
-    const std::string b = t + ".transformer_blocks.0";
-    for (int i = 0; i < 2; ++i)
-      m.attn.push_back(tattn(b + ".attention_blocks." + std::to_string(i), b + ".norms." + std::to_string(i), C));
-    m.ffn = norm(b + ".ff_norm", C, 1e-5f);
-    m.ff1 = ff1_geglu(b + ".ff.net.0.proj", C);
-    m.ff2 = lin(b + ".ff.net.2", C, 4 * C);
+    m.block = tblock(t + ".transformer_blocks.0", C, cfg.heads, 2);
     return m;
   }
 
-  // layer j: a resnet ins[j] -> C channels, then a transformer if j < n_attn and a motion module if j < n_mm
-  Stage stage(const std::string& name, const std::vector<int>& ins, int C, int temb, size_t n_attn, size_t n_mm) {
+  // layer j: a resnet ins[j] -> C channels (GroupNorm eps), then a transformer if j < n_attn and a motion module if j < n_mm
+  Stage stage(const std::string& name, const std::vector<int>& ins, int C, int temb, size_t n_attn, size_t n_mm, float eps = 1e-5f) {
     Stage s;
     s.name = name;
     for (size_t j = 0; j < ins.size(); ++j) {
       const std::string sj = "." + std::to_string(j);
-      s.res.push_back(resnet(name + ".resnets" + sj, ins[j], C, temb));
+      s.res.push_back(resnet(name + ".resnets" + sj, ins[j], C, temb, eps));
       if (j < n_attn) s.attn.push_back(spatial(name + ".attentions" + sj, C));
       if (j < n_mm) s.mm.push_back(motion(name + ".motion_modules" + sj, C));
     }
@@ -569,16 +586,7 @@ struct hv_model {
       r.block1 = conv3(p + ".block1", C, C);
       r.block2 = lin(p + ".block2", C, C);
       cam_res.push_back(r);
-      const std::string a = "encoder_down_attention_blocks.0." + std::to_string(j);
-      MotionW m;
-      m.C = C;
-      m.heads = cfg.cam_heads;
-      m.d = C / cfg.cam_heads;
-      m.attn.push_back(tattn(a + ".attention_blocks.0", a + ".norms.0", C));
-      m.ffn = norm(a + ".ff_norm", C, 1e-5f);
-      m.ff1 = ff1_geglu(a + ".ff.net.0.proj", C);
-      m.ff2 = lin(a + ".ff.net.2", C, 4 * C);
-      cam_att.push_back(m);
+      cam_att.push_back(tblock("encoder_down_attention_blocks.0." + std::to_string(j), C, cfg.cam_heads, 1));
     }
     cam_zero = lin("zero_conv_layers.0", C, C, false);
   }
@@ -596,29 +604,11 @@ struct hv_model {
     if (bias) l.bias = vec(pfx + ".bias", n, n_pad);
     return l;
   }
-  VaeAttnW vae_attn(const std::string& pfx, int C) {
+  // the mid block's attention (and its GroupNorm) of half `pfx`
+  void vae_attn(VaeHalf& v, const std::string& pfx, int C) {
     if (C != 512) fail(HV_ERR_INVALID, "'%s': the mid-block attention is implemented for 512 channels (one head of d = 512), got %d", pfx.c_str(), C);
-    VaeAttnW a;
-    a.gn = norm(pfx + ".group_norm", C, 1e-6f);
-    a.wqk = Mat{dmalloc(2LL * C * C), 2LL * C, C};
-    a.bqk = dmalloc(2LL * C);
-    const char* qk[2] = {".to_q", ".to_k"};
-    for (int i = 0; i < 2; ++i) {
-      ck(cudaMemcpyAsync(a.wqk.p + static_cast<int64_t>(i) * C * C, mat(pfx + qk[i] + ".weight", C, C).p, static_cast<size_t>(C) * C * 2, cudaMemcpyDeviceToDevice, st),
-         "q/k concat");
-      ck(cudaMemcpyAsync(a.bqk + static_cast<int64_t>(i) * C, vec(pfx + qk[i] + ".bias", C), static_cast<size_t>(C) * 2, cudaMemcpyDeviceToDevice, st), "q/k bias concat");
-    }
-    a.wv = mat(pfx + ".to_v.weight", C, C);
-    a.bv = vec(pfx + ".to_v.bias", C);
-    a.out = lin(pfx + ".to_out.0", C, C);
-    return a;
-  }
-  // a stage of n resnets (the first one ins -> C, the others C -> C), GroupNorm eps 1e-6, no time embedding
-  Stage vae_stage(const std::string& name, int ins, int C, int n) {
-    Stage s;
-    s.name = name;
-    for (int j = 0; j < n; ++j) s.res.push_back(resnet(name + ".resnets." + std::to_string(j), j == 0 ? ins : C, C, 0, 1e-6f));
-    return s;
+    v.attn_gn = norm(pfx + ".group_norm", C, 1e-6f);
+    v.attn = self_attn(pfx + ".to_q", pfx + ".to_k", pfx + ".to_v", pfx + ".to_out.0", C, 1, true);
   }
   void build_vae() {
     const int* ch = cfg.block_out_channels;
@@ -632,14 +622,14 @@ struct hv_model {
     enc.blocks.clear();
     int prev = ch[0];
     for (int i = 0; i < 4; ++i) {
-      Stage s = vae_stage("encoder.down_blocks." + std::to_string(i), prev, ch[i], 2);
+      Stage s = stage("encoder.down_blocks." + std::to_string(i), {prev, ch[i]}, ch[i], 0, 0, 0, 1e-6f);
       s.has_sampler = i < 3;
       if (s.has_sampler) s.sampler = conv3(s.name + ".downsamplers.0.conv", ch[i], ch[i]);
       enc.blocks.push_back(std::move(s));
       prev = ch[i];
     }
-    enc.mid = vae_stage("encoder.mid_block", ch[3], ch[3], 2);
-    enc.attn = vae_attn("encoder.mid_block.attentions.0", ch[3]);
+    enc.mid = stage("encoder.mid_block", {ch[3], ch[3]}, ch[3], 0, 0, 0, 1e-6f);
+    vae_attn(enc, "encoder.mid_block.attentions.0", ch[3]);
     enc.norm_out = norm("encoder.conv_norm_out", ch[3], 1e-6f);
     enc.conv_out = conv3("encoder.conv_out", 2 * zc, ch[3]);
     quant = lin("quant_conv", 2 * zc, 2 * zc);
@@ -647,13 +637,13 @@ struct hv_model {
     // 3x3 conv), conv_norm_out + SiLU, conv_out
     post_quant = padded_linear("post_quant_conv", zc, zc, 64, 64);
     dec.conv_in = conv3("decoder.conv_in", ch[3], zc);
-    dec.mid = vae_stage("decoder.mid_block", ch[3], ch[3], 2);
-    dec.attn = vae_attn("decoder.mid_block.attentions.0", ch[3]);
+    dec.mid = stage("decoder.mid_block", {ch[3], ch[3]}, ch[3], 0, 0, 0, 1e-6f);
+    vae_attn(dec, "decoder.mid_block.attentions.0", ch[3]);
     dec.blocks.clear();
     prev = ch[3];
     for (int i = 0; i < 4; ++i) {
       const int c = ch[3 - i];
-      Stage s = vae_stage("decoder.up_blocks." + std::to_string(i), prev, c, 3);
+      Stage s = stage("decoder.up_blocks." + std::to_string(i), {prev, c, c}, c, 0, 0, 0, 1e-6f);
       s.has_sampler = i < 3;
       if (s.has_sampler) s.sampler = upconv(s.name + ".upsamplers.0.conv", c, c);
       dec.blocks.push_back(std::move(s));
@@ -680,29 +670,14 @@ struct hv_model {
     clip_cls = vec(e + "class_embedding", C);
     clip_pos = mat(e + "position_embedding.weight", L, C).p;
     clip_pre = norm("vision_model.pre_layrnorm", C, eps);
-    clip_dv = static_cast<int>(rup(kClipHeadDim + 1, 16));
     clip_layers.clear();
     for (int i = 0; i < cfg.clip_layers; ++i) {
       const std::string pf = "vision_model.encoder.layers." + std::to_string(i) + ".";
       ClipLayerW w;
       w.ln1 = norm(pf + "layer_norm1", C, eps);
       w.ln2 = norm(pf + "layer_norm2", C, eps);
-      w.wqk = Mat{dmalloc(2LL * C * C), 2LL * C, C};
-      w.bqk = dmalloc(2LL * C);
-      const char* qk[2] = {"self_attn.q_proj", "self_attn.k_proj"};
-      for (int j = 0; j < 2; ++j) {
-        ck(cudaMemcpyAsync(w.wqk.p + static_cast<int64_t>(j) * C * C, mat(pf + qk[j] + ".weight", C, C).p, static_cast<size_t>(C) * C * 2,
-                           cudaMemcpyDeviceToDevice, st), "q/k concat");
-        ck(cudaMemcpyAsync(w.bqk + static_cast<int64_t>(j) * C, vec(pf + qk[j] + ".bias", C), static_cast<size_t>(C) * 2, cudaMemcpyDeviceToDevice, st),
-           "q/k bias concat");
-      }
-      w.wv = Mat{dmalloc(static_cast<int64_t>(heads) * clip_dv * C), static_cast<int64_t>(heads) * clip_dv, C};
-      ck(launch_pack_heads(mat(pf + "self_attn.v_proj.weight", C, C).p, w.wv.p, heads, kClipHeadDim, clip_dv, C, sms, st), "pack v");
-      // row bias of V^T: the ones rows, then v_proj's bias copied over the first d rows of every head
-      w.bv = vones(heads, clip_dv, kClipHeadDim);
-      ck(cudaMemcpy2DAsync(w.bv, static_cast<size_t>(clip_dv) * 2, vec(pf + "self_attn.v_proj.bias", C), kClipHeadDim * 2, kClipHeadDim * 2, heads,
-                           cudaMemcpyDeviceToDevice, st), "v bias pack");
-      w.out = lin(pf + "self_attn.out_proj", C, C);
+      const std::string a = pf + "self_attn.";
+      w.attn = self_attn(a + "q_proj", a + "k_proj", a + "v_proj", a + "out_proj", C, heads, true);
       w.fc1 = lin(pf + "mlp.fc1", I, C);
       w.fc2 = lin(pf + "mlp.fc2", C, I);
       clip_layers.push_back(w);
@@ -742,60 +717,73 @@ struct hv_model {
   }
   // frames per batch item the resnet / conv_norm_out GroupNorms pool their statistics over (use_inflated_groupnorm=False); 1 = per frame
   int gn_pool(int F) const { return (cfg.kind == HV_KIND_UNET3D && cfg.gn_pool_frames) ? F : 1; }
-  // out = LN(x (+ pre_add per batch item)) (+ pe per frame); returns the normalised tensor, x_new receives x + pre_add
-  Tens op_ln(const Tens& x, const Norm& n, const __half* pre_add, int64_t rows_per_b, Tens* x_new, const __half* pe, int F) {
+  // (B, C, F, H, W) -> channels-last (B * F, H, W, Cpad), channels C .. Cpad zero (an input read as one 64-wide k-block)
+  Tens padded_input(const __half* x, int B, int C, int F, int H, int W, int Cpad) {
+    Tens t = alloc_act(B * F, H, W, Cpad);
+    launch(2, {}, [&] {
+      ck(cudaMemsetAsync(t.p, 0, static_cast<size_t>(t.numel()) * 2, st), "memset");
+      ck(launch_ncfhw_to_nhwc(x, t.p, B, C, F, H, W, 0, st, Cpad), "input layout");
+    });
+    return t;
+  }
+  // out = LN(x (+ pre_add per batch item)) (+ pe per frame)
+  Tens op_ln(const Tens& x, const Norm& n, const __half* pre_add = nullptr, int64_t rows_per_b = 1, const __half* pe = nullptr, int F = 1) {
     Tens out = alloc_act(x.NF, x.H, x.W, x.C);
-    if (pre_add && x_new) *x_new = alloc_act(x.NF, x.H, x.W, x.C);
     launch(1, {CAT_NORM, "layernorm", 0, x.rows(), x.C, 0}, [&] {
-      ck(launch_layernorm(x.p, n.g, n.b, out.p, x.rows(), x.C, n.eps, pre_add, rows_per_b, (pre_add && x_new) ? x_new->p : nullptr, pe, x.H * x.W, F, st),
-         "layernorm");
+      ck(launch_layernorm(x.p, n.g, n.b, out.p, x.rows(), x.C, n.eps, pre_add, rows_per_b, nullptr, pe, x.H * x.W, F, st), "layernorm");
     });
     return out;
   }
-  void gemm(const __half* A, int64_t lda, const __half* A2, int64_t lda2, int64_t K1, const Mat& w, __half* out, int64_t ldc, int64_t M,
-            const hv_epilogue* ep) {
-    const char* label = (ep && ep->geglu) ? "gemm_geglu" : ((ep && ep->residual) ? "gemm_res" : "gemm");
-    launch(1, {CAT_GEMM, label, 2.0 * M * w.rows * w.cols, M, w.rows, w.cols},
-           [&] { ckop(op_gemm(A, lda, A2, lda2, K1, w.p, out, ldc, M, w.rows, w.cols, ep, st), "gemm"); });
+
+  // The GEMM / conv wrappers write into `dst` (a tensor of the output's shape allocated by the caller) or into a new tensor.  Their
+  // epilogue: + bias, + rowvec[row / rows_per_group] (rows of the output's width), act, + res.
+  Tens dest(const Tens* dst, int NF, int H, int W, int C) {
+    if (!dst) return alloc_act(NF, H, W, C);
+    if (dst->NF != NF || dst->H != H || dst->W != W || dst->C != C)
+      fail(HV_ERR_INVALID, "destination is (%d, %d, %d, %d), the output (%d, %d, %d, %d)", dst->NF, dst->H, dst->W, dst->C, NF, H, W, C);
+    return *dst;
   }
-  // y = x W^T + b (+ residual)
-  Tens op_linear(const Tens& x, const Lin& l, const Tens* residual, int act = HV_ACT_NONE, bool geglu = false) {
-    const int N = static_cast<int>(geglu ? l.w.rows / 2 : l.w.rows);
-    if (l.w.cols != x.C) fail(HV_ERR_INVALID, "linear: input width %d != weight cols %lld", x.C, (long long)l.w.cols);
-    Tens out = alloc_act(x.NF, x.H, x.W, N);
-    hv_epilogue ep{};
-    ep.bias = l.bias;
-    ep.act = act;
-    ep.geglu = geglu ? 1 : 0;
-    if (residual) { ep.residual = residual->p; ep.ldr = residual->C; }
-    gemm(x.p, x.C, nullptr, 0, 0, l.w, out.p, N, x.rows(), &ep);
+  static hv_epilogue epilogue(const __half* bias, const Tens* res, int act, const __half* rowvec, int64_t rows_per_group, int N) {
+    hv_epilogue e{};
+    e.bias = bias;
+    e.rowvec = rowvec;
+    e.rowvec_ld = N;
+    e.rows_per_group = static_cast<int32_t>(rows_per_group);
+    e.act = act;
+    if (res) { e.residual = res->p; e.ldr = res->C; }
+    return e;
+  }
+  // out = [x | x2] W^T + epilogue; x2: a second source concatenated along K (the skip tensor of a resnet shortcut)
+  Tens op_linear(const Tens& x, const Lin& l, const Tens* res = nullptr, const Tens* dst = nullptr, int act = HV_ACT_NONE, const Tens* x2 = nullptr,
+                 const __half* rowvec = nullptr, int64_t rows_per_group = 1) {
+    const int K1 = x2 ? x.C : 0, N = static_cast<int>(l.geglu ? l.w.rows / 2 : l.w.rows);
+    if (l.w.cols != x.C + (x2 ? x2->C : 0)) fail(HV_ERR_INVALID, "linear: input width %d + %d != weight cols %lld", x.C, x2 ? x2->C : 0, (long long)l.w.cols);
+    Tens out = dest(dst, x.NF, x.H, x.W, N);
+    hv_epilogue ep = epilogue(l.bias, res, act, rowvec, rows_per_group, N);
+    ep.geglu = l.geglu ? 1 : 0;
+    launch(1, {CAT_GEMM, l.geglu ? "gemm_geglu" : (res ? "gemm_res" : "gemm"), 2.0 * x.rows() * l.w.rows * l.w.cols, x.rows(), l.w.rows, l.w.cols}, [&] {
+      ckop(op_gemm(x.p, x.C, x2 ? x2->p : nullptr, x2 ? x2->C : 0, K1, l.w.p, out.p, out.C, x.rows(), l.w.rows, l.w.cols, &ep, st), "gemm");
+    });
     return out;
   }
   // pad_end: stride 2 with padding (0, 1, 0, 1) (AutoencoderKL's Downsample2D) instead of 1 on every side
-  Tens op_conv3(const Tens& x, const Conv3& c, int stride, const __half* rowvec, int64_t rows_per_group, int act, const Tens* residual,
-                bool pad_end = false) {
+  Tens op_conv3(const Tens& x, const Conv3& c, int stride = 1, const Tens* res = nullptr, const Tens* dst = nullptr, int act = HV_ACT_NONE,
+                const __half* rowvec = nullptr, int64_t rows_per_group = 1, bool pad_end = false) {
     if (x.C != c.cin_pad) fail(HV_ERR_INVALID, "conv3x3: input has %d channels, weight packed for %d", x.C, c.cin_pad);
     const int Ho = stride == 1 ? x.H : x.H / 2, Wo = stride == 1 ? x.W : x.W / 2;
-    Tens out = alloc_act(x.NF, Ho, Wo, c.cout_pad);
-    hv_epilogue ep{};
-    ep.bias = c.bias;
-    ep.rowvec = rowvec;
-    ep.rowvec_ld = c.cout_pad;
-    ep.rows_per_group = static_cast<int32_t>(rows_per_group);
-    ep.act = act;
-    if (residual) { ep.residual = residual->p; ep.ldr = residual->C; }
-    launch(1, {CAT_CONV, stride == 1 ? "conv3" : (pad_end ? "conv3_s2_end" : "conv3_s2"), 2.0 * out.rows() * c.cout * 9.0 * c.cin, out.rows(), c.cout_pad,
-               9LL * c.cin_pad},
-           [&] { ckop(op_conv3x3(x.p, c.w.p, out.p, c.cout_pad, x.NF, x.H, x.W, c.cin_pad, c.cout_pad, stride, &ep, st, pad_end), "conv3x3"); });
+    Tens out = dest(dst, x.NF, Ho, Wo, c.cout_pad);
+    const hv_epilogue ep = epilogue(c.bias, res, act, rowvec, rows_per_group, c.cout_pad);
+    const char* label = stride == 1 ? (res ? "conv3_res" : "conv3") : (pad_end ? "conv3_s2_end" : "conv3_s2");
+    launch(1, {CAT_CONV, label, 2.0 * out.rows() * c.cout * 9.0 * c.cin, out.rows(), c.cout_pad, 9LL * c.cin_pad},
+           [&] { ckop(op_conv3x3(x.p, c.w.p, out.p, out.C, x.NF, x.H, x.W, c.cin_pad, c.cout_pad, stride, &ep, st, pad_end), "conv3x3"); });
     return out;
   }
   // Upsample3D / Upsample2D: nearest 2x + 3x3 conv as four 2x2 convs of the source -- the 4x tensor is never materialised
-  Tens op_upconv(const Tens& h, const Conv3& c) {
-    Tens big = alloc_act(h.NF, 2 * h.H, 2 * h.W, c.cout);
-    hv_epilogue ep{};
-    ep.bias = c.bias;
+  Tens op_upconv(const Tens& h, const Conv3& c, const Tens* dst = nullptr) {
+    Tens big = dest(dst, h.NF, 2 * h.H, 2 * h.W, c.cout);
+    const hv_epilogue ep = epilogue(c.bias, nullptr, HV_ACT_NONE, nullptr, 1, c.cout);
     launch(1, {CAT_CONV, "upconv2x2", 2.0 * big.rows() * c.cout * 4.0 * c.cin, big.rows(), c.cout, 4LL * c.cin},
-           [&] { ckop(op_upconv2x2(h.p, c.w.p, big.p, c.cout, h.NF, h.H, h.W, c.cin, c.cout, &ep, st), "upsampler conv"); });
+           [&] { ckop(op_upconv2x2(h.p, c.w.p, big.p, big.C, h.NF, h.H, h.W, c.cin, c.cout, &ep, st), "upsampler conv"); });
     return big;
   }
   __half* op_small_linear(const __half* x, const Lin& l, int M, int act_in) {
@@ -818,25 +806,58 @@ struct hv_model {
     Scope s(ar);
     __half* tproj = r.has_temb ? op_small_linear(emb, r.temb, B, HV_ACT_SILU) : nullptr;  // time_emb_proj(silu(emb)) : [B][cout]
     Tens h = op_gn(x, x2, r.n1, true, gn_pool(F));
-    Tens h1 = op_conv3(h, r.c1, 1, tproj, static_cast<int64_t>(F) * x.H * x.W, HV_ACT_NONE, nullptr);
+    Tens h1 = op_conv3(h, r.c1, 1, nullptr, nullptr, HV_ACT_NONE, tproj, static_cast<int64_t>(F) * x.H * x.W);
     Tens h2 = op_gn(h1, nullptr, r.n2, true, gn_pool(F));
     Tens res = x;
-    if (r.has_sc) {
-      res = alloc_act(x.NF, x.H, x.W, r.cout);
-      hv_epilogue ep{};
-      ep.bias = r.sc.bias;
-      gemm(x.p, x.C, x2 ? x2->p : nullptr, x2 ? x2->C : 0, x2 ? x.C : 0, r.sc.w, res.p, r.cout, x.rows(), &ep);
-    } else if (x2) {
-      fail(HV_ERR_INVALID, "resnet with concatenated input must have a shortcut conv");
+    if (r.has_sc) res = op_linear(x, r.sc, nullptr, nullptr, HV_ACT_NONE, x2);
+    else if (x2) fail(HV_ERR_INVALID, "resnet with concatenated input must have a shortcut conv");
+    return op_conv3(h2, r.c2, 1, &res, &out);
+  }
+
+  // The reference bank a self-attention reads besides each frame's own tokens: keys [B][L][heads * dpad] and V^T with item i's tokens at
+  // columns i * vt_stride; frame n reads item n / F, the first nf_nobank frames read none.
+  struct BankKV {
+    const __half* k = nullptr;
+    const __half* vt = nullptr;
+    int L = 0, F = 1, nf_nobank = 0;
+    int64_t ldvt = 0, vt_stride = 0;
+  };
+  // Self-attention over each frame's H * W tokens of the normalised input xn: [Q | K] GEMM, V^T GEMM (frames side by side, its row bias
+  // the ones rows and v's bias), the attention kernel, out = to_out(.) + bias + res.  bank() runs between the V^T GEMM and the attention
+  // and returns the reference bank to read (the UNet's read / write hooks), or none.  The temporaries live in the caller's Scope.
+  template <class BankFn>
+  void self_attn_fwd(const SelfAttnW& a, const Tens& xn, const Tens& res, const Tens& out, BankFn&& bank) {
+    const int C = xn.C, L = xn.H * xn.W;
+    const int64_t hp = static_cast<int64_t>(a.heads) * a.dpad, Lp = rup(L, 8), ldvt = static_cast<int64_t>(xn.NF) * Lp;
+    const int64_t vrows = a.wv.rows;
+    Tens qk = op_linear(xn, a.qk);
+    __half* vt = alloc_h(vrows * ldvt);
+    // V^T[heads * dv][frame n: n * Lp + j] = Wv * xn^T: the weights are the "A" operand, the activations the batched "B" operand
+    launch(1, {CAT_GEMM, "gemm_vt", 2.0 * xn.rows() * C * C, vrows, xn.rows(), C},
+           [&] { ckop(op_gemm_batched_b(a.wv.p, C, xn.p, C, vt, ldvt, vrows, xn.NF, L, Lp, C, a.vbias, st), "V^T gemm"); });
+    const BankKV b = bank();
+    Tens o = alloc_act(xn.NF, xn.H, xn.W, C);
+    const double flops = 4.0 * L * a.heads * a.d * (static_cast<double>(xn.NF) * L + static_cast<double>(xn.NF - b.nf_nobank) * b.L);
+    if (a.dv == a.d) {   // single head, d = 512
+      if (b.L > 0) fail(HV_ERR_INVALID, "the d = 512 attention reads no reference bank");
+      launch(1, {CAT_ATTN, "attn_d512", flops, xn.NF, L, a.d}, [&] {
+        cudaError_t e = launch_attention_d512(qk.p, 2 * hp, qk.p + hp, 2 * hp, vt, ldvt, Lp, o.p, C, xn.NF, L, st);
+        if (e != cudaSuccess) fail(HV_ERR_CUDA, "attention d512: %s %s", cudaGetErrorString(e), tma_last_error());
+      });
+    } else {
+      launch(1, {CAT_ATTN, "attn", flops, xn.NF, L, a.d}, [&] {
+        AttnArgs g{};
+        g.q = qk.p; g.k = qk.p + hp; g.vt = vt; g.out = o.p;
+        g.NF = xn.NF; g.L = L; g.heads = a.heads; g.d = a.d; g.dpad = a.dpad;
+        g.ldq = 2 * hp; g.ldk = 2 * hp; g.ldvt = ldvt; g.ldo = C;
+        g.kb = b.k; g.vbt = b.vt; g.Lb = b.L; g.ldkb = hp; g.ldvbt = b.ldvt;
+        g.F = b.F; g.nf_nobank = b.nf_nobank;
+        g.vt_stride = Lp; g.vbt_stride = b.vt_stride;
+        cudaError_t e = launch_attention(g, sms, st);
+        if (e != cudaSuccess) fail(HV_ERR_CUDA, "attention (d = %d): %s %s", a.d, cudaGetErrorString(e), tma_last_error());
+      });
     }
-    // conv2 + bias, + residual, written straight into `out`
-    hv_epilogue ep{};
-    ep.bias = r.c2.bias;
-    ep.residual = res.p;
-    ep.ldr = res.C;
-    launch(1, {CAT_CONV, "conv3_res", 2.0 * x.rows() * r.cout * 9.0 * r.cout, x.rows(), r.cout, 9LL * r.c2.cin_pad},
-           [&] { ckop(op_conv3x3(h2.p, r.c2.w.p, out.p, r.cout, x.NF, x.H, x.W, r.c2.cin_pad, r.c2.cout_pad, 1, &ep, st), "resnet conv2"); });
-    return out;
+    op_linear(o, a.out, &res, &out);
   }
 
   // Transformer3DModel + TemporalBasicTransformerBlock (+ reference-bank read hook)
@@ -844,37 +865,26 @@ struct hv_model {
     Tens out = alloc_act(x.NF, x.H, x.W, x.C);
     Scope s(ar);
     const int C = w.C, L = x.H * x.W;
-    const int64_t tokens = x.rows();
     Tens hn = op_gn(x, nullptr, w.gn, false);
-    Tens t = op_linear(hn, w.proj_in, nullptr);
+    Tens t = op_linear(hn, w.proj_in);
     // ---- attn1
     Tens t1 = alloc_act(x.NF, x.H, x.W, C);  // t after self-attention residual
     {
       Scope s2(ar);
-      Tens n1 = op_ln(t, w.ln1, nullptr, 1, nullptr, nullptr, 1);
-      const int64_t hp = static_cast<int64_t>(w.heads) * w.dpad;
-      __half* qk = alloc_h(tokens * 2 * hp);
-      gemm(n1.p, C, nullptr, 0, 0, w.wqk, qk, 2 * hp, tokens, nullptr);
-      const int64_t Lp = rup(L, 8), ldvt = static_cast<int64_t>(x.NF) * Lp;
-      const int64_t vrows = static_cast<int64_t>(w.heads) * w.dv;
-      __half* vt = alloc_h(vrows * ldvt);
-      // V^T[C][frame n: n*Lp + j] = Wv [C][C] * n1^T : weights are the "A" operand, activations the batched "B" operand
-      launch(1, {CAT_GEMM, "gemm_vt", 2.0 * tokens * C * C, vrows, tokens, C},
-             [&] { ckop(op_gemm_batched_b(w.wv.p, C, n1.p, C, vt, ldvt, vrows, x.NF, L, Lp, C, w.vones, st), "V^T gemm"); });
-      // write hook (mutual_self_attention.py:137-146): the bank IS LayerNorm-1's output; attention then runs on itself only
-      if (bank_out != nullptr) {
-        launch(1, {}, [&] {
-          ck(cudaMemcpyAsync(bank_out[w.reader_idx], n1.p, static_cast<size_t>(tokens) * C * 2, cudaMemcpyDeviceToDevice, st), "bank write");
-        });
-      }
-      // HV_FLAG_CFG: batch = [uncond ; cond], the first half ignores the bank.  HV_FLAG_UNCOND_ONLY / HV_FLAG_COND_ONLY: the batch
-      // holds one CFG half only (a (window x CFG-half) unit of a multi-GPU split); a cond-only batch of B items reads the LAST B
-      // items of the bank (the bank is written for [uncond ; cond]).
-      const bool cfg_split = (flags & HV_FLAG_CFG) != 0 && B >= 2 && B % 2 == 0 && !(flags & (HV_FLAG_UNCOND_ONLY | HV_FLAG_COND_ONLY));
-      const bool use_bank = w.bank != nullptr && bank_out == nullptr && !(flags & HV_FLAG_UNCOND_ONLY);
-      __half *kb = nullptr, *vbt = nullptr;
-      int64_t ldvbt = 0, Lbp = 0;
-      if (use_bank) {
+      Tens n1 = op_ln(t, w.ln1);
+      self_attn_fwd(w.attn1, n1, t, t1, [&] {
+        BankKV b;
+        // write hook (mutual_self_attention.py:137-146): the bank IS LayerNorm-1's output; attention then runs on itself only
+        if (bank_out != nullptr) {
+          launch(1, {}, [&] {
+            ck(cudaMemcpyAsync(bank_out[w.reader_idx], n1.p, static_cast<size_t>(n1.numel()) * 2, cudaMemcpyDeviceToDevice, st), "bank write");
+          });
+        }
+        // HV_FLAG_CFG: batch = [uncond ; cond], the first half ignores the bank.  HV_FLAG_UNCOND_ONLY / HV_FLAG_COND_ONLY: the batch
+        // holds one CFG half only (a (window x CFG-half) unit of a multi-GPU split); a cond-only batch of B items reads the LAST B
+        // items of the bank (the bank is written for [uncond ; cond]).
+        const bool cfg_split = (flags & HV_FLAG_CFG) != 0 && B >= 2 && B % 2 == 0 && !(flags & (HV_FLAG_UNCOND_ONLY | HV_FLAG_COND_ONLY));
+        if (w.bank == nullptr || bank_out != nullptr || (flags & HV_FLAG_UNCOND_ONLY)) return b;
         int64_t item0 = 0;
         if (flags & HV_FLAG_COND_ONLY) {
           if (w.bank_B < B) fail(HV_ERR_INVALID, "reference bank of '%s' has batch %lld < forward batch %d", w.name.c_str(), (long long)w.bank_B, B);
@@ -882,62 +892,34 @@ struct hv_model {
         } else if (w.bank_B != B && !ar.dry) {   // (a planning pass only sizes the workspace; it does not know the flags of the forward to come)
           fail(HV_ERR_INVALID, "reference bank of '%s' has batch %lld, forward batch is %d", w.name.c_str(), (long long)w.bank_B, B);
         }
-        const __half* bank = w.bank + item0 * w.bank_L * C;
-        const int64_t bt = static_cast<int64_t>(B) * w.bank_L;
-        kb = alloc_h(bt * hp);
-        gemm(bank, C, nullptr, 0, 0, w.wk, kb, hp, bt, nullptr);
-        Lbp = rup(w.bank_L, 8);
-        ldvbt = static_cast<int64_t>(B) * Lbp;
-        vbt = alloc_h(vrows * ldvbt);
+        const SelfAttnW& a = w.attn1;
+        const int64_t hp = static_cast<int64_t>(a.heads) * a.dpad;
+        const Tens bank{w.bank + item0 * w.bank_L * C, B, 1, static_cast<int>(w.bank_L), C};
+        b.k = op_linear(bank, Lin{Mat{a.qk.w.p + hp * C, hp, C}}).p;   // the K rows of [Q | K] (the UNet's projections have no bias)
+        b.L = static_cast<int>(w.bank_L);
+        b.F = F;
+        b.nf_nobank = cfg_split ? (B / 2) * F : 0;
+        b.vt_stride = rup(w.bank_L, 8);
+        b.ldvt = static_cast<int64_t>(B) * b.vt_stride;
+        __half* vbt = alloc_h(a.wv.rows * b.ldvt);
+        b.vt = vbt;
         // its profile row has no label and no shape, so bench.py's per-shape GEMM roofline (gemm_classes) leaves it out
-        launch(1, {CAT_GEMM, "", 2.0 * bt * C * C},
-               [&] { ckop(op_gemm_batched_b(w.wv.p, C, bank, C, vbt, ldvbt, vrows, B, w.bank_L, Lbp, C, w.vones, st), "bank V^T gemm"); });
-      }
-      Tens o = alloc_act(x.NF, x.H, x.W, C);
-      const int Lb = use_bank ? static_cast<int>(w.bank_L) : 0, nf_nobank = cfg_split ? (B / 2) * F : 0;
-      launch(1, {CAT_ATTN, "attn", 4.0 * L * w.C * (static_cast<double>(x.NF) * L + static_cast<double>(x.NF - nf_nobank) * Lb), x.NF, L, w.d}, [&] {
-        AttnArgs a{};
-        a.q = qk; a.k = qk + hp; a.vt = vt; a.out = o.p;
-        a.NF = x.NF; a.L = L; a.heads = w.heads; a.d = w.d; a.dpad = w.dpad;
-        a.ldq = 2 * hp; a.ldk = 2 * hp; a.ldvt = ldvt; a.ldo = C;
-        a.kb = kb; a.vbt = vbt; a.Lb = Lb; a.ldkb = hp; a.ldvbt = ldvbt;
-        a.F = F; a.nf_nobank = nf_nobank;
-        a.vt_stride = Lp; a.vbt_stride = Lbp;
-        cudaError_t e = launch_attention(a, sms, st);
-        if (e != cudaSuccess) fail(HV_ERR_CUDA, "attention (%s): %s %s", w.name.c_str(), cudaGetErrorString(e), tma_last_error());
+        launch(1, {CAT_GEMM, "", 2.0 * bank.rows() * C * C}, [&] {
+          ckop(op_gemm_batched_b(a.wv.p, C, bank.p, C, vbt, b.ldvt, a.wv.rows, B, w.bank_L, b.vt_stride, C, a.vbias, st), "bank V^T gemm");
+        });
+        return b;
       });
-      hv_epilogue ep{};
-      ep.bias = w.out1.bias;
-      ep.residual = t.p;
-      ep.ldr = C;
-      gemm(o.p, C, nullptr, 0, 0, w.out1.w, t1.p, C, tokens, &ep);
     }
     // ---- attn2 with a single key: softmax == 1 -> out = to_out(to_v(ehs_b)) for every token of batch item b
     __half* v2 = op_small_linear(ehs, w.v2, B, HV_ACT_NONE);
     __half* ca = op_small_linear(v2, w.out2, B, HV_ACT_NONE);
     // LayerNorm-3 normalises t2 = t1 + ca[b] without writing t2: the same per-batch vector is added again, in fp32, in FF2's epilogue
     // (t3 = ff2(.) + bias + ca[b] + t1), which saves one full-tensor write per block and one rounding of the residual stream
-    Tens n3 = op_ln(t1, w.ln3, ca, static_cast<int64_t>(F) * L, nullptr, nullptr, 1);
-    // ---- feed-forward
-    Tens ffh = op_linear(n3, w.ff1, nullptr, HV_ACT_NONE, true);
-    Tens t3 = alloc_act(x.NF, x.H, x.W, C);
-    {
-      hv_epilogue ep{};
-      ep.bias = w.ff2.bias;
-      ep.rowvec = ca;
-      ep.rowvec_ld = C;
-      ep.rows_per_group = static_cast<int32_t>(static_cast<int64_t>(F) * L);
-      ep.residual = t1.p;
-      ep.ldr = C;
-      gemm(ffh.p, ffh.C, nullptr, 0, 0, w.ff2.w, t3.p, C, tokens, &ep);
-    }
-    // ---- proj_out + residual
-    hv_epilogue ep{};
-    ep.bias = w.proj_out.bias;
-    ep.residual = x.p;
-    ep.ldr = x.C;
-    gemm(t3.p, C, nullptr, 0, 0, w.proj_out.w, out.p, C, tokens, &ep);
-    return out;
+    Tens n3 = op_ln(t1, w.ln3, ca, static_cast<int64_t>(F) * L);
+    // ---- feed-forward, proj_out + residual
+    Tens ffh = op_linear(n3, w.ff1);
+    Tens t3 = op_linear(ffh, w.ff2, &t1, nullptr, HV_ACT_NONE, nullptr, ca, static_cast<int64_t>(F) * L);
+    return op_linear(t3, w.proj_out, &x, &out);
   }
 
   // one temporal attention sub-block: t = to_out(attn(LN(t) + pe)) + t
@@ -946,18 +928,19 @@ struct hv_model {
     Tens out = alloc_act(t.NF, t.H, t.W, t.C);
     Scope s(ar);
     const int C = t.C;
-    Tens n = op_ln(t, a.ln, nullptr, 1, nullptr, a.pe, F);
-    __half* qkv = alloc_h(t.rows() * 3 * C);
-    gemm(n.p, C, nullptr, 0, 0, a.wqkv, qkv, 3 * C, t.rows(), nullptr);
+    Tens n = op_ln(t, a.ln, nullptr, 1, a.pe, F);
+    Tens qkv = op_linear(n, a.qkv);
     Tens o = alloc_act(t.NF, t.H, t.W, C);
     launch(1, {CAT_TATTN, "tattn", 4.0 * t.rows() * F * C, t.rows(), F, C},
-           [&] { ck(launch_temporal_attention(qkv, o.p, B, F, t.H * t.W, heads, d, st), "temporal attention"); });
-    hv_epilogue ep{};
-    ep.bias = a.out.bias;
-    ep.residual = t.p;
-    ep.ldr = C;
-    gemm(o.p, C, nullptr, 0, 0, a.out.w, out.p, C, t.rows(), &ep);
-    return out;
+           [&] { ck(launch_temporal_attention(qkv.p, o.p, B, F, t.H * t.W, heads, d, st), "temporal attention"); });
+    return op_linear(o, a.out, &t, &out);
+  }
+  // TemporalTransformerBlock: the temporal attentions, then t = ff(LN(t)) + t
+  Tens tblock_fwd(const TBlockW& b, Tens t, int B, int F) {
+    for (const auto& a : b.attn) t = tattn_fwd(a, t, B, F, b.heads, b.d);
+    Tens n = op_ln(t, b.ff_norm);
+    Tens ffh = op_linear(n, b.ff1);
+    return op_linear(ffh, b.ff2, &t);
   }
 
   // VanillaTemporalModule (motion_module.py:44-259)
@@ -965,17 +948,9 @@ struct hv_model {
     Tens out = alloc_act(x.NF, x.H, x.W, x.C);
     Scope s(ar);
     Tens hn = op_gn(x, nullptr, m.gn, false);
-    Tens t = op_linear(hn, m.proj_in, nullptr);
-    for (const auto& a : m.attn) t = tattn_fwd(a, t, B, F, m.heads, m.d);
-    Tens n = op_ln(t, m.ffn, nullptr, 1, nullptr, nullptr, 1);
-    Tens ffh = op_linear(n, m.ff1, nullptr, HV_ACT_NONE, true);
-    Tens t2 = op_linear(ffh, m.ff2, &t);
-    hv_epilogue ep{};
-    ep.bias = m.proj_out.bias;
-    ep.residual = x.p;
-    ep.ldr = x.C;
-    gemm(t2.p, x.C, nullptr, 0, 0, m.proj_out.w, out.p, x.C, x.rows(), &ep);
-    return out;
+    Tens t = op_linear(hn, m.proj_in);
+    Tens t2 = tblock_fwd(m.block, t, B, F);
+    return op_linear(t2, m.proj_out, &x, &out);
   }
 
   // ================================================================== forwards
@@ -1007,15 +982,11 @@ struct hv_model {
     launch(1, {}, [&] { ck(launch_timestep_embedding(timestep, ts_table, ts_index, tsin, B, ch[0], st), "timestep embedding"); });
     __half* e1 = op_small_linear(tsin, te1, B, HV_ACT_NONE);
     __half* emb = op_small_linear(e1, te2, B, HV_ACT_SILU);
-    // conv_in (+ pose_cond_fea as the epilogue residual); the 4 latent channels are zero-padded to one 64-wide k-block
-    Tens x0 = alloc_act(NF, H, W, conv_in.cin_pad);
+    // conv_in (+ pose_cond_fea as the epilogue residual)
+    Tens x0 = padded_input(sample, B, cfg.in_channels, F, H, W, conv_in.cin_pad);
     Tens pc = pose ? alloc_act(NF, H, W, ch[0]) : Tens{};
-    launch(2 + (pose ? 1 : 0), {}, [&] {
-      ck(cudaMemsetAsync(x0.p, 0, static_cast<size_t>(x0.numel()) * 2, st), "memset");
-      ck(launch_ncfhw_to_nhwc(sample, x0.p, B, cfg.in_channels, F, H, W, 0, st, x0.C), "sample layout");
-      if (pose) ck(launch_ncfhw_to_nhwc(pose, pc.p, B, ch[0], F, H, W, 0, st), "pose layout");
-    });
-    Tens h = op_conv3(x0, conv_in, 1, nullptr, 1, HV_ACT_NONE, pose ? &pc : nullptr);
+    if (pose) launch(1, {}, [&] { ck(launch_ncfhw_to_nhwc(pose, pc.p, B, ch[0], F, H, W, 0, st), "pose layout"); });
+    Tens h = op_conv3(x0, conv_in, 1, pose ? &pc : nullptr);
     tap("conv_in", h);
     // layer j of stage s (skip: the down-path tensor an up-path resnet concatenates)
     auto layer = [&](const Stage& s, size_t j, const Tens* skip) {
@@ -1032,7 +1003,7 @@ struct hv_model {
         skips.push_back(h);
       }
       if (s.has_sampler) {
-        h = op_conv3(h, s.sampler, 2, nullptr, 1, HV_ACT_NONE, nullptr);
+        h = op_conv3(h, s.sampler, 2);
         tap(s.name + ".downsamplers.0", h);
         skips.push_back(h);
       }
@@ -1055,7 +1026,7 @@ struct hv_model {
       return;
     }
     Tens hn = op_gn(h, nullptr, norm_out, true, gn_pool(F));
-    Tens y = op_conv3(hn, conv_out, 1, nullptr, 1, HV_ACT_NONE, nullptr);
+    Tens y = op_conv3(hn, conv_out);
     launch(1, {}, [&] { ck(launch_nhwc_to_ncfhw(y.p, y.C, outp, B, cfg.out_channels, F, H, W, st), "output layout"); });
   }
 
@@ -1092,7 +1063,7 @@ struct hv_model {
         h = out;
         continue;
       }
-      h = op_conv3(h, c, pg_strides[i], nullptr, 1, last ? HV_ACT_NONE : HV_ACT_SILU, nullptr);
+      h = op_conv3(h, c, pg_strides[i], nullptr, nullptr, last ? HV_ACT_NONE : HV_ACT_SILU);
       // the next conv expects cin_pad channels: cout_pad of this conv equals it by construction (both round to 64)
       if (!last && h.C != pg_convs[i + 1].cin_pad) fail(HV_ERR_INVALID, "pose guider channel padding mismatch at conv %zu", i);
     }
@@ -1111,93 +1082,56 @@ struct hv_model {
       else
         ck(launch_pixel_unshuffle(plucker, u.p, B, cin0, F, H, W, r, sms, st), "pixel unshuffle");
     });
-    Tens x = op_conv3(u, cam_in, 1, nullptr, 1, HV_ACT_NONE, nullptr);
+    Tens x = op_conv3(u, cam_in);
     for (int j = 0; j < cfg.cam_nums_rb; ++j) {
       // ResnetBlock (pose_adaptor.py:102-135, sk=True, ksize=1): x = block2(relu(block1(x))) + x
-      Tens h1 = op_conv3(x, cam_res[j].block1, 1, nullptr, 1, HV_ACT_RELU, nullptr);
+      Tens h1 = op_conv3(x, cam_res[j].block1, 1, nullptr, nullptr, HV_ACT_RELU);
       x = op_linear(h1, cam_res[j].block2, &x);
-      // TemporalTransformerBlock over the frame axis
-      const MotionW& m = cam_att[j];
-      Tens t = tattn_fwd(m.attn[0], x, B, F, m.heads, m.d);
-      Tens n = op_ln(t, m.ffn, nullptr, 1, nullptr, nullptr, 1);
-      Tens ffh = op_linear(n, m.ff1, nullptr, HV_ACT_NONE, true);
-      x = op_linear(ffh, m.ff2, &t);
+      x = tblock_fwd(cam_att[j], x, B, F);   // over the frame axis
     }
-    Tens z = op_linear(x, cam_zero, nullptr);
+    Tens z = op_linear(x, cam_zero);
     launch(1, {}, [&] { ck(launch_nhwc_to_ncfhw(z.p, z.C, outp, NF, C, 1, z.H, z.W, st), "camera output layout"); });
   }
 
   // ================================================================== AutoencoderKL
-  // diffusers Attention of the VAE mid block: GroupNorm -> q, k, v (+bias) -> one head of d = 512 -> to_out (+bias) + residual.  Q and
-  // K come from one GEMM, V^T (frames side by side) from the swapped GEMM with to_v's bias as its row bias.
-  Tens vae_attn_fwd(const VaeAttnW& w, const Tens& x) {
-    Tens out = alloc_act(x.NF, x.H, x.W, x.C);
-    Scope s(ar);
-    const int C = x.C, L = x.H * x.W;
-    const int64_t tokens = x.rows();
-    Tens hn = op_gn(x, nullptr, w.gn, false);
-    __half* qk = alloc_h(tokens * 2 * C);
-    hv_epilogue eqk{};
-    eqk.bias = w.bqk;
-    gemm(hn.p, C, nullptr, 0, 0, w.wqk, qk, 2 * C, tokens, &eqk);
-    const int64_t Lp = rup(L, 8), ldvt = static_cast<int64_t>(x.NF) * Lp;
-    __half* vt = alloc_h(C * ldvt);
-    launch(1, {CAT_GEMM, "gemm_vt", 2.0 * tokens * C * C, C, tokens, C},
-           [&] { ckop(op_gemm_batched_b(w.wv.p, C, hn.p, C, vt, ldvt, C, x.NF, L, Lp, C, w.bv, st), "V^T gemm"); });
-    Tens o = alloc_act(x.NF, x.H, x.W, C);
-    launch(1, {CAT_ATTN, "attn_d512", 4.0 * x.NF * static_cast<double>(L) * L * C, x.NF, L, C}, [&] {
-      cudaError_t e = launch_attention_d512(qk, 2 * C, qk + C, 2 * C, vt, ldvt, Lp, o.p, C, x.NF, L, st);
-      if (e != cudaSuccess) fail(HV_ERR_CUDA, "attention d512: %s %s", cudaGetErrorString(e), tma_last_error());
-    });
-    hv_epilogue ep{};
-    ep.bias = w.out.bias;
-    ep.residual = x.p;
-    ep.ldr = x.C;
-    gemm(o.p, C, nullptr, 0, 0, w.out.w, out.p, C, tokens, &ep);
-    return out;
-  }
-  // UNetMidBlock2D: resnet, attention, resnet
+  // UNetMidBlock2D: resnet, attention (diffusers Attention: GroupNorm, self-attention + residual), resnet
   Tens vae_mid_fwd(const VaeHalf& v, Tens h) {
     h = resnet_fwd(v.mid.res[0], h, nullptr, nullptr, h.NF, 1);
-    h = vae_attn_fwd(v.attn, h);
-    return resnet_fwd(v.mid.res[1], h, nullptr, nullptr, h.NF, 1);
+    Tens a = alloc_act(h.NF, h.H, h.W, h.C);
+    {
+      Scope s(ar);
+      self_attn_fwd(v.attn, op_gn(h, nullptr, v.attn_gn, false), h, a, [] { return BankKV{}; });
+    }
+    return resnet_fwd(v.mid.res[1], a, nullptr, nullptr, a.NF, 1);
   }
   // Every operator works per frame (per-frame GroupNorm statistics, per-frame attention), so frame i of a call does not depend on the
   // other frames of the call.
   void vae_encode(const __half* x, __half* moments, int N, int H, int W) {
     if (N <= 0 || H <= 0 || W <= 0 || (H % 8) || (W % 8)) fail(HV_ERR_INVALID, "AutoencoderKL.encode: N = %d images of %dx%d: N must be > 0 and H, W positive multiples of 8", N, H, W);
-    Tens x0 = alloc_act(N, H, W, enc.conv_in.cin_pad);   // the image channels zero-padded to one 64-wide k-block
-    launch(2, {}, [&] {
-      ck(cudaMemsetAsync(x0.p, 0, static_cast<size_t>(x0.numel()) * 2, st), "memset");
-      ck(launch_ncfhw_to_nhwc(x, x0.p, N, cfg.in_channels, 1, H, W, 0, st, x0.C), "image layout");
-    });
-    Tens h = op_conv3(x0, enc.conv_in, 1, nullptr, 1, HV_ACT_NONE, nullptr);
+    Tens x0 = padded_input(x, N, cfg.in_channels, 1, H, W, enc.conv_in.cin_pad);
+    Tens h = op_conv3(x0, enc.conv_in);
     for (const Stage& s : enc.blocks) {
       for (const ResnetW& r : s.res) h = resnet_fwd(r, h, nullptr, nullptr, N, 1);
-      if (s.has_sampler) h = op_conv3(h, s.sampler, 2, nullptr, 1, HV_ACT_NONE, nullptr, true);   // Downsample2D: pad (0, 1, 0, 1), stride 2
+      if (s.has_sampler) h = op_conv3(h, s.sampler, 2, nullptr, nullptr, HV_ACT_NONE, nullptr, 1, true);   // Downsample2D: pad (0, 1, 0, 1), stride 2
     }
     h = vae_mid_fwd(enc, h);
     Tens hn = op_gn(h, nullptr, enc.norm_out, true);
-    Tens y = op_conv3(hn, enc.conv_out, 1, nullptr, 1, HV_ACT_NONE, nullptr);
-    Tens m = op_linear(y, quant, nullptr);   // quant_conv (1x1)
+    Tens y = op_conv3(hn, enc.conv_out);
+    Tens m = op_linear(y, quant);   // quant_conv (1x1)
     launch(1, {}, [&] { ck(launch_nhwc_to_ncfhw(m.p, m.C, moments, N, m.C, 1, m.H, m.W, st), "moments layout"); });
   }
   void vae_decode(const __half* z, __half* outp, int N, int H, int W) {
     if (N <= 0 || H <= 0 || W <= 0) fail(HV_ERR_INVALID, "AutoencoderKL.decode: N = %d latents of %dx%d must all be positive", N, H, W);
-    Tens z0 = alloc_act(N, H, W, static_cast<int>(post_quant.w.cols));   // latent channels zero-padded to 64
-    launch(2, {}, [&] {
-      ck(cudaMemsetAsync(z0.p, 0, static_cast<size_t>(z0.numel()) * 2, st), "memset");
-      ck(launch_ncfhw_to_nhwc(z, z0.p, N, cfg.vae_latent_channels, 1, H, W, 0, st, z0.C), "latent layout");
-    });
-    Tens p = op_linear(z0, post_quant, nullptr);   // post_quant_conv (1x1); its padded channels stay zero for conv_in
-    Tens h = op_conv3(p, dec.conv_in, 1, nullptr, 1, HV_ACT_NONE, nullptr);
+    Tens z0 = padded_input(z, N, cfg.vae_latent_channels, 1, H, W, static_cast<int>(post_quant.w.cols));
+    Tens p = op_linear(z0, post_quant);   // post_quant_conv (1x1); its padded channels stay zero for conv_in
+    Tens h = op_conv3(p, dec.conv_in);
     h = vae_mid_fwd(dec, h);
     for (const Stage& s : dec.blocks) {
       for (const ResnetW& r : s.res) h = resnet_fwd(r, h, nullptr, nullptr, N, 1);
       if (s.has_sampler) h = op_upconv(h, s.sampler);
     }
     Tens hn = op_gn(h, nullptr, dec.norm_out, true);
-    Tens y = op_conv3(hn, dec.conv_out, 1, nullptr, 1, HV_ACT_NONE, nullptr);
+    Tens y = op_conv3(hn, dec.conv_out);
     launch(1, {}, [&] { ck(launch_nhwc_to_ncfhw(y.p, y.C, outp, N, cfg.out_channels, 1, y.H, y.W, st), "image output layout"); });
   }
 
@@ -1207,41 +1141,14 @@ struct hv_model {
   // quick-GELU -> fc2 + bias + residual.
   void clip_layer_fwd(const ClipLayerW& w, const Tens& x, __half* out) {
     Scope s(ar);
-    const int C = x.C, L = x.W, heads = cfg.clip_heads;
-    const int64_t tokens = x.rows();
-    Tens n1 = op_ln(x, w.ln1, nullptr, 1, nullptr, nullptr, 1);
-    __half* qk = alloc_h(tokens * 2 * C);
-    hv_epilogue eqk{};
-    eqk.bias = w.bqk;
-    gemm(n1.p, C, nullptr, 0, 0, w.wqk, qk, 2 * C, tokens, &eqk);
-    const int64_t Lp = rup(L, 8), ldvt = static_cast<int64_t>(x.NF) * Lp, vrows = w.wv.rows;
-    __half* vt = alloc_h(vrows * ldvt);
-    launch(1, {CAT_GEMM, "gemm_vt", 2.0 * tokens * C * C, vrows, tokens, C},
-           [&] { ckop(op_gemm_batched_b(w.wv.p, C, n1.p, C, vt, ldvt, vrows, x.NF, L, Lp, C, w.bv, st), "V^T gemm"); });
-    Tens o = alloc_act(x.NF, x.H, x.W, C);
-    launch(1, {CAT_ATTN, "attn", 4.0 * L * C * static_cast<double>(x.NF) * L, x.NF, L, kClipHeadDim}, [&] {
-      AttnArgs a{};
-      a.q = qk; a.k = qk + C; a.vt = vt; a.out = o.p;
-      a.NF = x.NF; a.L = L; a.heads = heads; a.d = kClipHeadDim; a.dpad = kClipHeadDim;
-      a.ldq = 2 * C; a.ldk = 2 * C; a.ldvt = ldvt; a.ldo = C;
-      a.F = 1; a.nf_nobank = 0;
-      a.vt_stride = Lp;
-      cudaError_t e = launch_attention(a, sms, st);
-      if (e != cudaSuccess) fail(HV_ERR_CUDA, "CLIP attention: %s %s", cudaGetErrorString(e), tma_last_error());
-    });
-    Tens h1 = alloc_act(x.NF, x.H, x.W, C);
-    hv_epilogue eo{};
-    eo.bias = w.out.bias;
-    eo.residual = x.p;
-    eo.ldr = C;
-    gemm(o.p, C, nullptr, 0, 0, w.out.w, h1.p, C, tokens, &eo);
-    Tens n2 = op_ln(h1, w.ln2, nullptr, 1, nullptr, nullptr, 1);
-    Tens f = op_linear(n2, w.fc1, nullptr, HV_ACT_QUICK_GELU);
-    hv_epilogue e2{};
-    e2.bias = w.fc2.bias;
-    e2.residual = h1.p;
-    e2.ldr = C;
-    gemm(f.p, f.C, nullptr, 0, 0, w.fc2.w, out, C, tokens, &e2);
+    Tens n1 = op_ln(x, w.ln1);
+    Tens h1 = alloc_act(x.NF, x.H, x.W, x.C);
+    self_attn_fwd(w.attn, n1, x, h1, [] { return BankKV{}; });
+    Tens n2 = op_ln(h1, w.ln2);
+    Tens f = op_linear(n2, w.fc1, nullptr, nullptr, HV_ACT_QUICK_GELU);
+    Tens y = x;
+    y.p = out;
+    op_linear(f, w.fc2, &h1, &y);
   }
   // pixels (B, 3, S, S) -> image_embeds (B, projection_dim) and, if lhs != nullptr, last_hidden_state (B, L, hidden).  Every operator works per
   // token row, per (image, head) or per output element, so image i of a call does not depend on the other images.
@@ -1251,10 +1158,9 @@ struct hv_model {
            cfg.clip_image_size);
     const int C = cfg.clip_hidden_size, p = cfg.clip_patch_size, np = (S / p) * (S / p), L = np + 1, Kpad = clip_kpad();
     // patch embedding: the stride-p conv as patchify + GEMM
-    __half* prow = alloc_h(static_cast<int64_t>(B) * np * Kpad);
-    launch(1, {}, [&] { ck(launch_clip_patchify(pix, prow, B, 3, S, p, Kpad, sms, st), "patchify"); });
-    Tens pe = alloc_act(B, 1, np, C);
-    gemm(prow, Kpad, nullptr, 0, 0, clip_patch.w, pe.p, C, pe.rows(), nullptr);
+    Tens prow = alloc_act(B, 1, np, Kpad);
+    launch(1, {}, [&] { ck(launch_clip_patchify(pix, prow.p, B, 3, S, p, Kpad, sms, st), "patchify"); });
+    Tens pe = op_linear(prow, clip_patch);
     // [class_embedding ; patches] + position_embedding -> pre_layrnorm: the residual stream (B images x L tokens)
     Tens x = alloc_act(B, 1, L, C);
     launch(1, {CAT_NORM, "clip_embed_ln", 0, x.rows(), C, 0},
@@ -1271,7 +1177,7 @@ struct hv_model {
       ck(cudaMemcpy2DAsync(cls.p, static_cast<size_t>(C) * 2, x.p, static_cast<size_t>(L) * C * 2, static_cast<size_t>(C) * 2, B, cudaMemcpyDeviceToDevice, st),
          "class tokens");
     });
-    Tens pooled = op_ln(cls, clip_post, nullptr, 1, nullptr, nullptr, 1);
+    Tens pooled = op_ln(cls, clip_post);
     const int P = static_cast<int>(clip_proj.rows);
     launch(1, {CAT_MISC, "", 2.0 * B * P * C},
            [&] { ck(launch_small_linear(pooled.p, clip_proj.p, nullptr, embeds, B, P, C, HV_ACT_NONE, st), "visual_projection"); });
