@@ -22,7 +22,7 @@
 #include <math.h>
 #include <stdint.h>
 
-#include "kernels.h"
+#include "ops.h"
 #include "ptx.cuh"
 #include "tma.h"
 #include "wgmma.cuh"
@@ -37,6 +37,16 @@ constexpr float kRescaleThreshold = 8.0f;  // log2 units: O is rescaled only whe
 constexpr int ATT_THREADS = 384;
 constexpr int kMathWarps = 8;
 constexpr uint32_t kProducerRegs = 40, kMathRegs = 232;
+
+struct AttnArgs {
+  const __half* q; const __half* k; const __half* vt; __half* out;
+  int NF, L, heads, d, dpad;
+  long long ldq, ldk, ldvt, ldo;
+  const __half* kb; const __half* vbt;   // bank keys [B][Lb][ldkb], bank values transposed [heads*d][ldvbt]
+  int Lb; long long ldkb, ldvbt;
+  int F, nf_nobank;
+  long long vt_stride, vbt_stride;       // columns between consecutive frames / bank items in V^T (multiples of 8)
+};
 
 template <int D>
 struct ACfg {
@@ -327,7 +337,7 @@ attn_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ C
 }
 
 template <int D>
-cudaError_t launch_attn_t(const AttnArgs& a, cudaStream_t stream) {
+int launch_attn_t(const AttnArgs& a, cudaStream_t stream) {
   using C = ACfg<D>;
   static_assert(C::kStages >= 1, "one K/V stage must fit in shared memory");
   CUtensorMap mq, mk, mvt, mkb, mvbt;
@@ -335,16 +345,17 @@ cudaError_t launch_attn_t(const AttnArgs& a, cudaStream_t stream) {
   // the maps span the heads * dpad columns that exist: the last head's 64-column box then ends in TMA's zero fill instead of
   // reading past the row (past the buffer's end for K's last token, where K sits after Q in an interleaved row)
   const long long cols = static_cast<long long>(a.heads) * C::kDpad;
-  if (!make_map_2d(&mq, a.q, tokens, cols, a.ldq, QT)) return cudaErrorInvalidValue;
-  if (!make_map_2d(&mk, a.k, tokens, cols, a.ldk, KT)) return cudaErrorInvalidValue;
-  if (!make_map_2d(&mvt, a.vt, static_cast<long long>(a.heads) * C::kDv, static_cast<long long>(a.NF) * a.vt_stride, a.ldvt, C::kDv)) return cudaErrorInvalidValue;
+  bool maps = make_map_2d(&mq, a.q, tokens, cols, a.ldq, QT) && make_map_2d(&mk, a.k, tokens, cols, a.ldk, KT) &&
+              make_map_2d(&mvt, a.vt, static_cast<long long>(a.heads) * C::kDv, static_cast<long long>(a.NF) * a.vt_stride, a.ldvt, C::kDv);
   mkb = mk;
   mvbt = mvt;
   const int B = a.NF / (a.F > 0 ? a.F : 1);
-  if (a.Lb > 0) {
-    if (!make_map_2d(&mkb, a.kb, static_cast<long long>(B) * a.Lb, a.ldkb, a.ldkb, KT)) return cudaErrorInvalidValue;
-    if (!make_map_2d(&mvbt, a.vbt, static_cast<long long>(a.heads) * C::kDv, static_cast<long long>(B) * a.vbt_stride, a.ldvbt, C::kDv))
-      return cudaErrorInvalidValue;
+  if (maps && a.Lb > 0)
+    maps = make_map_2d(&mkb, a.kb, static_cast<long long>(B) * a.Lb, a.ldkb, a.ldkb, KT) &&
+           make_map_2d(&mvbt, a.vbt, static_cast<long long>(a.heads) * C::kDv, static_cast<long long>(B) * a.vbt_stride, a.ldvbt, C::kDv);
+  if (!maps) {
+    set_error("hv_op_attention (d = %d) map: %s", D, tma_last_error());
+    return HV_ERR_TMA;
   }
   AttnKernelArgs ka;
   ka.out = a.out;
@@ -360,26 +371,55 @@ cudaError_t launch_attn_t(const AttnArgs& a, cudaStream_t stream) {
   static bool attr = false;
   if (!attr) {
     cudaError_t e = cudaFuncSetAttribute(attn_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes);
-    if (e != cudaSuccess) return e;
+    if (e != cudaSuccess) return cuda_status(e, "hv_op_attention");
     attr = true;
   }
   dim3 grid((a.L + QT - 1) / QT, a.heads, a.NF);
   attn_kernel<D><<<grid, ATT_THREADS, C::kSmemBytes, stream>>>(mq, mk, mvt, mkb, mvbt, ka);
-  return cudaGetLastError();
+  return cuda_status(cudaGetLastError(), "hv_op_attention");
 }
 
 }  // namespace
 
-cudaError_t launch_attention(const AttnArgs& a, int /*num_sms*/, cudaStream_t stream) {
-  switch (a.d) {
+int op_attention(const __half* Q, const __half* K, const __half* Vt, __half* out, int64_t NF, int64_t L, int heads, int d, int64_t ldq,
+                 int64_t ldk, int64_t ldvt, int64_t ldo, const __half* Kb, const __half* Vbt, int64_t Lb, int64_t ldkb, int64_t ldvbt, int64_t F,
+                 int64_t nf_nobank, int64_t vt_stride, int64_t vbt_stride, cudaStream_t stream) {
+  if ((vt_stride % 8) || (vbt_stride % 8) || vt_stride < L) { set_error("hv_op_attention: V^T frame strides must be multiples of 8 and >= L"); return HV_ERR_INVALID; }
+  if ((ldq % 8) || (ldk % 8) || (ldvt % 8) || (ldo % 8) || (d % 8)) { set_error("hv_op_attention: strides / head dim must be multiples of 8"); return HV_ERR_INVALID; }
+  // every token, V^T column and TMA coordinate below is an int, and NF / heads are grid dimensions (<= 65535)
+  const bool d_ok = d == 8 || d == 16 || d == 32 || d == 40 || d == 64 || d == 80 || d == 160;
+  const int64_t dpad = (d + 15) / 16 * 16;
+  if (!Q || !K || !Vt || !out || NF < 1 || NF > 65535 || L < 1 || L > INT32_MAX || vt_stride > INT32_MAX || heads < 1 || heads > 65535 || !d_ok ||
+      NF * L > INT32_MAX || NF * vt_stride > INT32_MAX || nf_nobank < 0 || nf_nobank > NF || ldo < heads * d || ldq < heads * dpad || ldk < heads * dpad ||
+      ldvt < NF * vt_stride) {
+    set_error("hv_op_attention: bad arguments NF=%lld L=%lld heads=%d d=%d ldq=%lld ldk=%lld ldvt=%lld ldo=%lld vt_stride=%lld nf_nobank=%lld "
+              "(pointers non-NULL, 1 <= NF, heads <= 65535, 0 <= nf_nobank <= NF, ldo >= heads*d, ldq and ldk >= heads*dpad, ldvt >= NF*vt_stride)",
+              (long long)NF, (long long)L, heads, d, (long long)ldq, (long long)ldk, (long long)ldvt, (long long)ldo, (long long)vt_stride,
+              (long long)nf_nobank);
+    return HV_ERR_INVALID;
+  }
+  const bool bank = Kb != nullptr && Lb > 0;   // a NULL Kb (or Lb = 0) means no bank, whatever the other bank arguments hold
+  if (bank && (!Vbt || F < 1 || NF % F || Lb > INT32_MAX || vbt_stride > INT32_MAX || vbt_stride < Lb || NF / F * Lb > INT32_MAX || NF / F * vbt_stride > INT32_MAX || ldkb < heads * dpad ||
+               (ldkb % 8) || (ldvbt % 8) || ldvbt < NF / F * vbt_stride)) {
+    set_error("hv_op_attention: bad bank arguments NF=%lld F=%lld Lb=%lld ldkb=%lld ldvbt=%lld vbt_stride=%lld (Vbt non-NULL, F divides NF, "
+              "vbt_stride >= Lb, ldkb >= heads*dpad, ldvbt >= (NF/F)*vbt_stride)", (long long)NF, (long long)F, (long long)Lb, (long long)ldkb,
+              (long long)ldvbt, (long long)vbt_stride);
+    return HV_ERR_INVALID;
+  }
+  AttnArgs a;
+  a.q = Q; a.k = K; a.vt = Vt; a.out = out;
+  a.NF = (int)NF; a.L = (int)L; a.heads = heads; a.d = d; a.dpad = (int)dpad;  // V^T rows per head: (d + 1 + 15) / 16 * 16, row d of every head = ones
+  a.ldq = ldq; a.ldk = ldk; a.ldvt = ldvt; a.ldo = ldo;
+  a.kb = Kb; a.vbt = Vbt; a.Lb = bank ? (int)Lb : 0; a.ldkb = ldkb; a.ldvbt = ldvbt;
+  a.F = (int)F; a.nf_nobank = (int)nf_nobank; a.vt_stride = vt_stride; a.vbt_stride = vbt_stride;
+  switch (d) {
     case 8: return launch_attn_t<8>(a, stream);
     case 16: return launch_attn_t<16>(a, stream);
     case 32: return launch_attn_t<32>(a, stream);
     case 40: return launch_attn_t<40>(a, stream);
     case 64: return launch_attn_t<64>(a, stream);
     case 80: return launch_attn_t<80>(a, stream);
-    case 160: return launch_attn_t<160>(a, stream);
-    default: return cudaErrorInvalidValue;
+    default: return launch_attn_t<160>(a, stream);   // d_ok above
   }
 }
 

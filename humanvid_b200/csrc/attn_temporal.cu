@@ -12,7 +12,7 @@
 #include <stdint.h>
 #include <stdlib.h>
 
-#include "kernels.h"
+#include "ops.h"
 #include "ptx.cuh"
 #include "tma.h"
 
@@ -390,32 +390,45 @@ temporal_attn_tma_kernel(const __grid_constant__ CUtensorMap map_qkv, const __gr
 }
 
 template <int D, int HPB>
-static cudaError_t launch_tt(const __half* qkv, __half* out, int B, int F, int HW, int heads, float scale_log2, unsigned grid, cudaStream_t stream) {
+static int launch_tt(const __half* qkv, __half* out, int B, int F, int HW, int heads, float scale_log2, unsigned grid, cudaStream_t stream) {
   using C = TTCfg<D, HPB>;
   const int Cc = heads * D;
   CUtensorMap mq, mo;
-  if (!make_map_frames(&mq, qkv, static_cast<int64_t>(B) * F, HW, 3LL * Cc, 3LL * Cc, D * HPB, F)) return cudaErrorInvalidValue;
-  if (!make_map_frames(&mo, out, static_cast<int64_t>(B) * F, HW, Cc, Cc, D * HPB, F)) return cudaErrorInvalidValue;
+  if (!make_map_frames(&mq, qkv, static_cast<int64_t>(B) * F, HW, 3LL * Cc, 3LL * Cc, D * HPB, F) ||
+      !make_map_frames(&mo, out, static_cast<int64_t>(B) * F, HW, Cc, Cc, D * HPB, F)) {
+    set_error("hv_op_temporal_attention map: %s", tma_last_error());
+    return HV_ERR_TMA;
+  }
   static bool attr = false;
   if (!attr) {
     cudaError_t e = cudaFuncSetAttribute(temporal_attn_tma_kernel<D, HPB>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes);
-    if (e != cudaSuccess) return e;
+    if (e != cudaSuccess) return cuda_status(e, "hv_op_temporal_attention");
     attr = true;
   }
   temporal_attn_tma_kernel<D, HPB><<<grid, TT_WARPS * 32, C::kSmemBytes, stream>>>(mq, mo, B, F, HW, heads, scale_log2);
-  return cudaGetLastError();
+  return cuda_status(cudaGetLastError(), "hv_op_temporal_attention");
 }
 
 constexpr int kRegWarpsPerBlock = 8;
 
 }  // namespace
 
-TemporalPlan plan_temporal_attention(int B, int HW, int heads, int d, int sms) {
-  TemporalPlan p;
-  const long long nprob = static_cast<long long>(B) * HW * heads;
+// rows (b, f, p) and the one-warp-per-problem grid of the register kernel are indexed with ints
+int plan_temporal_attention(const char* what, int64_t B, int64_t F, int64_t HW, int heads, int d, TemporalPlan* plan) {
+  const bool d_ok = d == 8 || d == 16 || d == 32 || d == 40 || d == 80 || d == 160;
+  if (B < 1 || B > INT32_MAX || F < 1 || F > 32 || HW < 1 || HW > INT32_MAX || heads < 1 || !d_ok || B * F > INT32_MAX || B * F * HW > INT32_MAX ||
+      B * HW * heads > INT32_MAX || static_cast<int64_t>(heads) * d * 3 > INT32_MAX) {
+    set_error("%s: bad shape B=%lld F=%lld HW=%lld heads=%d d=%d (B, HW, heads >= 1, 1 <= F <= 32, d one of 8, 16, 32, 40, 80, 160)", what,
+              (long long)B, (long long)F, (long long)HW, heads, d);
+    return HV_ERR_INVALID;
+  }
+  const int sms = device_sms();
+  if (!sms) return HV_ERR_CUDA;
+  TemporalPlan& p = *plan;
+  const long long nprob = B * HW * heads;
   // the two high-resolution levels; small problems keep the register kernel.  The choice depends on HW only, not on the batch size
   // (a one-half unit of the multi-GPU split must run the same kernel as that half of a CFG batch).
-  if (static_cast<long long>(HW) * heads >= 2048 && ((d == 40 && heads % 2 == 0) || d == 80)) {
+  if (HW * heads >= 2048 && ((d == 40 && heads % 2 == 0) || d == 80)) {
     p.tma = true;
     p.heads_per_box = d == 40 ? 2 : 1;
     const long long ctas = (nprob / p.heads_per_box + TT_WARPS - 1) / TT_WARPS;   // persistent: at most one CTA per SM
@@ -425,18 +438,14 @@ TemporalPlan plan_temporal_attention(int B, int HW, int heads, int d, int sms) {
     p.heads_per_box = 1;
     p.grid = static_cast<unsigned>((nprob + kRegWarpsPerBlock - 1) / kRegWarpsPerBlock);
   }
-  return p;
+  return HV_OK;
 }
 
-cudaError_t launch_temporal_attention(const __half* qkv, __half* out, int B, int F, int HW, int heads, int d, cudaStream_t stream) {
-  if (F < 1 || F > 32) return cudaErrorInvalidValue;
-  static int sms = 0;
-  if (!sms) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  }
-  const TemporalPlan plan = plan_temporal_attention(B, HW, heads, d, sms);
+int op_temporal_attention(const __half* qkv, __half* out, int64_t B64, int64_t F64, int64_t HW64, int heads, int d, cudaStream_t stream) {
+  if (!qkv || !out) { set_error("hv_op_temporal_attention: NULL pointer"); return HV_ERR_INVALID; }
+  TemporalPlan plan;
+  if (int rc = plan_temporal_attention("hv_op_temporal_attention", B64, F64, HW64, heads, d, &plan)) return rc;
+  const int B = static_cast<int>(B64), F = static_cast<int>(F64), HW = static_cast<int>(HW64);
   const unsigned grid = plan.grid;
   const int wpb = kRegWarpsPerBlock;
   const float scale_log2 = 1.4426950408889634f / sqrtf(static_cast<float>(d));
@@ -450,10 +459,9 @@ cudaError_t launch_temporal_attention(const __half* qkv, __half* out, int B, int
     case 160: temporal_attn_kernel<160><<<grid, wpb * 32, 0, stream>>>(qkv, out, B, F, HW, heads, scale_log2); break;
     case 32: temporal_attn_kernel<32><<<grid, wpb * 32, 0, stream>>>(qkv, out, B, F, HW, heads, scale_log2); break;
     case 16: temporal_attn_kernel<16><<<grid, wpb * 32, 0, stream>>>(qkv, out, B, F, HW, heads, scale_log2); break;
-    case 8: temporal_attn_kernel<8><<<grid, wpb * 32, 0, stream>>>(qkv, out, B, F, HW, heads, scale_log2); break;
-    default: return cudaErrorInvalidValue;
+    default: temporal_attn_kernel<8><<<grid, wpb * 32, 0, stream>>>(qkv, out, B, F, HW, heads, scale_log2); break;   // d = 8 (checked above)
   }
-  return cudaGetLastError();
+  return cuda_status(cudaGetLastError(), "hv_op_temporal_attention");
 }
 
 }  // namespace hv

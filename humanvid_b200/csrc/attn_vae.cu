@@ -20,7 +20,7 @@
 #include <math.h>
 #include <stdint.h>
 
-#include "kernels.h"
+#include "ops.h"
 #include "ptx.cuh"
 #include "tma.h"
 #include "wgmma.cuh"
@@ -207,26 +207,33 @@ attn_d512_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constan
 
 }  // namespace
 
-cudaError_t launch_attention_d512(const __half* q, long long ldq, const __half* k, long long ldk, const __half* vt, long long ldvt, long long vt_stride,
-                                  __half* out, long long ldo, int NF, int L, cudaStream_t stream) {
-  if (NF <= 0 || L <= 0 || NF > 65535) return cudaErrorInvalidValue;
+int op_attention_d512(const __half* q, int64_t ldq, const __half* k, int64_t ldk, const __half* vt, int64_t ldvt, int64_t vt_stride, __half* out,
+                      int64_t ldo, int64_t NF, int64_t L, cudaStream_t stream) {
+  if (!q || !k || !vt || !out || NF <= 0 || NF > 65535 || L <= 0 || L > (1 << 24) || (ldq % 8) || (ldk % 8) || (ldvt % 8) || (ldo % 8) ||
+      (vt_stride % 8) || vt_stride < L || ldq < 512 || ldk < 512 || ldo < 512) {
+    set_error("hv_op_attention_d512: bad shape NF=%lld L=%lld ldq=%lld ldk=%lld ldvt=%lld vt_stride=%lld ldo=%lld (strides multiples of 8, rows >= 512 wide, "
+              "vt_stride >= L)", (long long)NF, (long long)L, (long long)ldq, (long long)ldk, (long long)ldvt, (long long)vt_stride, (long long)ldo);
+    return HV_ERR_INVALID;
+  }
   CUtensorMap mq, mk, mvt;
-  if (!make_map_3d(&mq, q, NF, L, D, ldq, QT)) return cudaErrorInvalidValue;
-  if (!make_map_3d(&mk, k, NF, L, D, ldk, KT)) return cudaErrorInvalidValue;
-  if (!make_map_col_batches(&mvt, vt, NF, D, L, ldvt, vt_stride, D / 2)) return cudaErrorInvalidValue;
+  if (!make_map_3d(&mq, q, NF, L, D, ldq, QT) || !make_map_3d(&mk, k, NF, L, D, ldk, KT) ||
+      !make_map_col_batches(&mvt, vt, NF, D, L, ldvt, vt_stride, D / 2)) {
+    set_error("hv_op_attention_d512 map: %s", tma_last_error());
+    return HV_ERR_TMA;
+  }
   D512Args ka;
   ka.out = out;
   ka.ldo = ldo;
-  ka.L = L;
+  ka.L = static_cast<int>(L);
   ka.scale_log2 = 1.4426950408889634f / sqrtf(static_cast<float>(D));
   static bool attr = false;
   if (!attr) {
     cudaError_t e = cudaFuncSetAttribute(attn_d512_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
-    if (e != cudaSuccess) return e;
+    if (e != cudaSuccess) return cuda_status(e, "hv_op_attention_d512");
     attr = true;
   }
-  attn_d512_kernel<<<dim3((L + QT - 1) / QT, NF), kThreads, kSmemBytes, stream>>>(mq, mk, mvt, ka);
-  return cudaGetLastError();
+  attn_d512_kernel<<<dim3(static_cast<unsigned>((L + QT - 1) / QT), static_cast<unsigned>(NF)), kThreads, kSmemBytes, stream>>>(mq, mk, mvt, ka);
+  return cuda_status(cudaGetLastError(), "hv_op_attention_d512");
 }
 
 }  // namespace hv

@@ -538,11 +538,7 @@ bool plan_gemm(const GemmProblem& p, int block_n, int num_sms, GemmPlan* plan) {
 }
 
 cudaError_t launch_gemm(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const CUtensorMap& out, const CUtensorMap& res,
-                        const GemmProblem& p, const GemmEpilogue& e, int block_n, int num_sms, cudaStream_t stream) {
-  GemmPlan plan;
-  if (!plan_gemm(p, block_n, num_sms, &plan)) return cudaErrorInvalidValue;
-  if (p.b_batch && (e.bias || e.rowvec || e.residual || e.geglu || (p.b_out_stride % 8))) return cudaErrorInvalidValue;
-  if (e.geglu && block_n != 256) return cudaErrorInvalidValue;
+                        const GemmProblem& p, const GemmEpilogue& e, int block_n, const GemmPlan& plan, cudaStream_t stream) {
   if (plan.bst_stages > 0) {
     if (block_n == 256) return launch_t<256, true>(a0, a1, b, out, res, p, e, plan, stream);
     if (block_n == 160) return launch_t<160, true>(a0, a1, b, out, res, p, e, plan, stream);

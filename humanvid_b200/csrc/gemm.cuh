@@ -63,9 +63,9 @@ bool plan_gemm(const GemmProblem& p, int block_n, int num_sms, GemmPlan* plan);
 // a0/a1: TMA maps of the A operand with 128-row boxes (see make_* helpers in tma.h), b: TMA map of the packed weights [N][K].
 // out / res: make_map_tile_* maps of e.out (ldc) and e.residual (ldr) over the written region [0, n_valid) x rows (linear: 2-D,
 // 3x3 conv: 4-D over the output grid); unused by the up-convolution and batched-B paths, and res unused without a residual.
-// block_n must be 128, 160 or 256 (256 required for geglu); 160 = two exact tiles for the 320-wide layers.
+// block_n must be 128, 160 or 256 (256 required for geglu); 160 = two exact tiles for the 320-wide layers.  plan: plan_gemm(p, block_n).
 cudaError_t launch_gemm(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const CUtensorMap& out, const CUtensorMap& res,
-                        const GemmProblem& p, const GemmEpilogue& e, int block_n, int num_sms, cudaStream_t stream);
+                        const GemmProblem& p, const GemmEpilogue& e, int block_n, const GemmPlan& plan, cudaStream_t stream);
 
 // Picks the (bn, bh, bw) output-tile box of 128 output pixels with the least padding for an NF x H x W output
 // (every box dimension is a power of two <= 128).

@@ -5,6 +5,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "ops.h"
 #include "ptx.cuh"
 
 namespace hv {
@@ -280,90 +281,148 @@ __global__ void clip_patchify_kernel(const __half* __restrict__ x, __half* __res
 
 }  // namespace
 
-#define HV_LAUNCH_CHECK() return cudaGetLastError()
-
-cudaError_t launch_clip_patchify(const __half* x, __half* out, int B, int Cin, int S, int p, int Kpad, int num_sms, cudaStream_t s) {
-  if (B <= 0 || Cin <= 0 || p <= 0 || S <= 0 || S % p || Kpad < Cin * p * p) return cudaErrorInvalidValue;
-  const long long total = static_cast<long long>(B) * (S / p) * (S / p) * Kpad;
-  clip_patchify_kernel<<<blocks_for(total, num_sms), kThreads, 0, s>>>(x, out, total, Cin, S, p, Kpad);
-  HV_LAUNCH_CHECK();
+// Each operator below rejects NULL pointers and sizes its kernel would narrow out of int32 (or, where a size becomes gridDim.y / .z,
+// past 65535) before it launches; the message lists what the operator needs.
+static int invalid(const char* op, const char* needs) {
+  set_error("%s: bad arguments (%s)", op, needs);
+  return HV_ERR_INVALID;
 }
 
-cudaError_t launch_ncfhw_to_nhwc(const void* x, __half* out, int B, int C, int F, int H, int W, int src_fp32, cudaStream_t s, int ldo) {
+int op_clip_patchify(const __half* x, __half* out, int64_t B, int64_t Cin, int64_t S, int64_t p, int64_t Kpad, cudaStream_t s) {
+  if (!x || !out || B <= 0 || Cin <= 0 || p <= 0 || S <= 0 || (S % p) || (Kpad % 8) || Kpad < Cin * p * p || Kpad > INT32_MAX || B * S * S * Cin > INT32_MAX) {
+    set_error("hv_op_clip_patchify: bad shape B=%lld C=%lld S=%lld p=%lld Kpad=%lld (S %% p == 0, Kpad >= C p^2 and a multiple of 8)", (long long)B,
+              (long long)Cin, (long long)S, (long long)p, (long long)Kpad);
+    return HV_ERR_INVALID;
+  }
+  const int sms = device_sms();
+  if (!sms) return HV_ERR_CUDA;
+  const long long total = B * (S / p) * (S / p) * Kpad;
+  clip_patchify_kernel<<<blocks_for(total, sms), kThreads, 0, s>>>(x, out, total, static_cast<int>(Cin), static_cast<int>(S), static_cast<int>(p),
+                                                                     static_cast<int>(Kpad));
+  return cuda_status(cudaGetLastError(), "hv_op_clip_patchify");
+}
+
+// the tiled transposes: (C + 31) / 32 tiles and B * F frames are the grid's y and z dimensions
+static bool transpose_ok(int64_t B, int64_t C, int64_t F, int64_t H, int64_t W) {
+  return B >= 1 && F >= 1 && B * F <= 65535 && C >= 1 && (C + 31) / 32 <= 65535 && H >= 1 && W >= 1 && H * W <= INT32_MAX;
+}
+
+int op_ncfhw_to_nhwc(const void* x, __half* out, int64_t B, int64_t C, int64_t F, int64_t H, int64_t W, int src_fp32, cudaStream_t s, int64_t ldo) {
   if (ldo <= 0) ldo = C;
-  const int HW = H * W;
-  dim3 grid((HW + 31) / 32, (C + 31) / 32, B * F), block(32, 8);
+  if (!x || !out || !transpose_ok(B, C, F, H, W) || ldo < C || ldo > INT32_MAX)
+    return invalid("hv_op_ncfhw_to_nhwc", "non-NULL pointers, B, C, F, H, W >= 1, B*F <= 65535, H*W and ldo >= C within int32");
+  const int HW = static_cast<int>(H * W);
+  dim3 grid((HW + 31) / 32, static_cast<unsigned>((C + 31) / 32), static_cast<unsigned>(B * F)), block(32, 8);
   if (src_fp32)
-    ncfhw_to_nhwc_kernel<float><<<grid, block, 0, s>>>(static_cast<const float*>(x), out, B, C, F, HW, ldo);
+    ncfhw_to_nhwc_kernel<float><<<grid, block, 0, s>>>(static_cast<const float*>(x), out, static_cast<int>(B), static_cast<int>(C), static_cast<int>(F), HW,
+                                                       static_cast<int>(ldo));
   else
-    ncfhw_to_nhwc_kernel<__half><<<grid, block, 0, s>>>(static_cast<const __half*>(x), out, B, C, F, HW, ldo);
-  HV_LAUNCH_CHECK();
+    ncfhw_to_nhwc_kernel<__half><<<grid, block, 0, s>>>(static_cast<const __half*>(x), out, static_cast<int>(B), static_cast<int>(C), static_cast<int>(F), HW,
+                                                        static_cast<int>(ldo));
+  return cuda_status(cudaGetLastError(), "hv_op_ncfhw_to_nhwc");
 }
-cudaError_t launch_nhwc_to_ncfhw(const __half* x, int ldx, __half* out, int B, int C, int F, int H, int W, cudaStream_t s) {
-  const int HW = H * W;
-  dim3 grid((HW + 31) / 32, (C + 31) / 32, B * F), block(32, 8);
-  nhwc_to_ncfhw_kernel<<<grid, block, 0, s>>>(x, ldx, out, B, C, F, HW);
-  HV_LAUNCH_CHECK();
+int op_nhwc_to_ncfhw(const __half* x, int64_t ldx, __half* out, int64_t B, int64_t C, int64_t F, int64_t H, int64_t W, cudaStream_t s) {
+  if (!x || !out || !transpose_ok(B, C, F, H, W) || ldx < C || ldx > INT32_MAX)
+    return invalid("hv_op_nhwc_to_ncfhw", "non-NULL pointers, B, C, F, H, W >= 1, B*F <= 65535, H*W and ldx >= C within int32");
+  const int HW = static_cast<int>(H * W);
+  dim3 grid((HW + 31) / 32, static_cast<unsigned>((C + 31) / 32), static_cast<unsigned>(B * F)), block(32, 8);
+  nhwc_to_ncfhw_kernel<<<grid, block, 0, s>>>(x, static_cast<int>(ldx), out, static_cast<int>(B), static_cast<int>(C), static_cast<int>(F), HW);
+  return cuda_status(cudaGetLastError(), "hv_op_nhwc_to_ncfhw");
 }
-cudaError_t launch_pixel_unshuffle(const __half* x, __half* out, int B, int C, int F, int H, int W, int r, int num_sms, cudaStream_t s) {
-  const long long total = static_cast<long long>(B) * F * C * H * W;
-  pixel_unshuffle_kernel<<<blocks_for(total, num_sms), kThreads, 0, s>>>(x, out, total, B, C, F, H, W, r);
-  HV_LAUNCH_CHECK();
+int op_pixel_unshuffle(const __half* x, __half* out, int64_t B, int64_t C, int64_t F, int64_t H, int64_t W, int r, cudaStream_t s) {
+  if (!x || !out || !int32_ok(B) || !int32_ok(F) || !int32_ok(B * F) || !int32_ok(H) || !int32_ok(W) || r < 1 || (H % r) || (W % r) ||
+      !int32_ok(C * r * r))
+    return invalid("hv_op_pixel_unshuffle", "non-NULL pointers, r >= 1 dividing H and W, B, C, F, H, W >= 1, B*F and C*r*r within int32");
+  const int sms = device_sms();
+  if (!sms) return HV_ERR_CUDA;
+  const long long total = B * F * C * H * W;
+  pixel_unshuffle_kernel<<<blocks_for(total, sms), kThreads, 0, s>>>(x, out, total, static_cast<int>(B), static_cast<int>(C), static_cast<int>(F),
+                                                                      static_cast<int>(H), static_cast<int>(W), r);
+  return cuda_status(cudaGetLastError(), "hv_op_pixel_unshuffle");
 }
-cudaError_t launch_plucker_unshuffle(const float* K, const float* c2w, __half* out, long long NF, int H, int W, int r, int num_sms, cudaStream_t s) {
+int op_plucker_unshuffle(const float* K, const float* c2w, __half* out, int64_t NF, int64_t H, int64_t W, int r, cudaStream_t s) {
+  if (!K || !c2w || !out || NF <= 0 || r < 1 || (H % r) || (W % r) || H > INT32_MAX || W > INT32_MAX)
+    return invalid("hv_op_plucker_unshuffle", "non-NULL pointers, NF >= 1, r >= 1 dividing H and W, H and W within int32");
+  const int sms = device_sms();
+  if (!sms) return HV_ERR_CUDA;
   const long long total = NF * H * W;
-  plucker_unshuffle_kernel<<<blocks_for(total, num_sms), kThreads, 0, s>>>(K, c2w, out, total, H, W, r);
-  HV_LAUNCH_CHECK();
+  plucker_unshuffle_kernel<<<blocks_for(total, sms), kThreads, 0, s>>>(K, c2w, out, total, static_cast<int>(H), static_cast<int>(W), r);
+  return cuda_status(cudaGetLastError(), "hv_op_plucker_unshuffle");
 }
-cudaError_t launch_small_linear(const __half* x, const __half* w, const __half* bias, __half* out, int M, int N, int K, int act_in,
-                                cudaStream_t s) {
-  const long long warps = static_cast<long long>(M) * N;
-  small_linear_kernel<<<static_cast<unsigned>((warps * 32 + kThreads - 1) / kThreads), kThreads, 0, s>>>(x, w, bias, out, M, N, K, act_in);
-  HV_LAUNCH_CHECK();
+// one warp per output element, x and w read as half2
+int op_small_linear(const __half* x, const __half* w, const __half* bias, __half* out, int64_t M, int64_t N, int64_t K, int act_in, cudaStream_t s) {
+  if (!x || !w || !out || (reinterpret_cast<uintptr_t>(x) & 3) || (reinterpret_cast<uintptr_t>(w) & 3) || !int32_ok(M) || !int32_ok(N) || !int32_ok(K) ||
+      (K % 2) || (M * N + 7) / 8 > INT32_MAX)
+    return invalid("hv_op_small_linear", "non-NULL, 4-byte aligned X and W, M, N >= 1, K >= 2 and even, M*N/8 blocks within int32");
+  const long long warps = M * N;
+  small_linear_kernel<<<static_cast<unsigned>((warps * 32 + kThreads - 1) / kThreads), kThreads, 0, s>>>(x, w, bias, out, static_cast<int>(M),
+                                                                                                         static_cast<int>(N), static_cast<int>(K), act_in);
+  return cuda_status(cudaGetLastError(), "hv_op_small_linear");
 }
-cudaError_t launch_timestep_embedding(long long timestep, const long long* table, const int* index, __half* out, int B, int dim, cudaStream_t s) {
-  const int n = B * dim / 2;
-  timestep_embedding_kernel<<<(n + 127) / 128, 128, 0, s>>>(static_cast<float>(timestep), table, index, out, B, dim);
-  HV_LAUNCH_CHECK();
+int op_timestep_embedding(int64_t timestep, const long long* table, const int* index, __half* out, int64_t B, int64_t dim, cudaStream_t s) {
+  if (!out || (table && !index) || B < 1 || dim < 2 || (dim % 2) || B * dim > INT32_MAX)
+    return invalid("hv_op_timestep_embedding", "non-NULL out, B >= 1, dim >= 2 and even, B*dim within int32");
+  const int n = static_cast<int>(B * dim / 2);
+  timestep_embedding_kernel<<<(n + 127) / 128, 128, 0, s>>>(static_cast<float>(timestep), table, index, out, static_cast<int>(B), static_cast<int>(dim));
+  return cuda_status(cudaGetLastError(), "hv_op_timestep_embedding");
 }
-cudaError_t launch_conv3x3_direct(const __half* x, const __half* w, const __half* bias, __half* out, long long NF, int H, int W, int Cin,
-                                  int Cout, int stride, int act, const __half* add, int num_sms, cudaStream_t s) {
-  const int Ho = (H - 1) / stride + 1, Wo = (W - 1) / stride + 1;
+int op_conv3x3_direct(const __half* x, const __half* w, const __half* bias, __half* out, int64_t NF, int64_t H, int64_t W, int64_t Cin, int64_t Cout,
+                      int stride, int act, const __half* add, int64_t ldo, cudaStream_t s) {
+  if (!x || !w || !out || NF < 1 || !int32_ok(H) || !int32_ok(W) || !int32_ok(Cin) || !int32_ok(Cout) || (stride != 1 && stride != 2) || ldo < Cout ||
+      ldo > INT32_MAX)
+    return invalid("hv_op_conv3x3_direct", "non-NULL X, W and out, stride 1 or 2, NF, H, W, Cin, Cout >= 1 within int32, Cout <= ldo within int32");
+  const int sms = device_sms();
+  if (!sms) return HV_ERR_CUDA;
+  const int Hi = static_cast<int>(H), Wi = static_cast<int>(W), Ho = (Hi - 1) / stride + 1, Wo = (Wi - 1) / stride + 1;
   const long long total = NF * Ho * Wo * ((Cout + 7) / 8);
-  conv3x3_direct_kernel<<<blocks_for(total, num_sms), kThreads, 0, s>>>(x, w, bias, out, total, H, W, Cin, Cout, stride, act, add, Cout);
-  HV_LAUNCH_CHECK();
+  conv3x3_direct_kernel<<<blocks_for(total, sms), kThreads, 0, s>>>(x, w, bias, out, total, Hi, Wi, static_cast<int>(Cin), static_cast<int>(Cout), stride,
+                                                                     act, add, static_cast<int>(ldo));
+  return cuda_status(cudaGetLastError(), "hv_op_conv3x3_direct");
 }
-// same, writing into a channel-padded buffer (row stride ldo >= Cout; the pad channels must already be zero)
-cudaError_t launch_conv3x3_direct_padded(const __half* x, const __half* w, const __half* bias, __half* out, long long NF, int H, int W,
-                                         int Cin, int Cout, int ldo, int act, int num_sms, cudaStream_t s) {
-  const long long total = NF * H * W * ((Cout + 7) / 8);
-  conv3x3_direct_kernel<<<blocks_for(total, num_sms), kThreads, 0, s>>>(x, w, bias, out, total, H, W, Cin, Cout, 1, act, nullptr, ldo);
-  HV_LAUNCH_CHECK();
+int op_pack_conv3x3(const __half* w, __half* out, int64_t Cout, int64_t Cin, int64_t Cout_pad, int64_t Cin_pad, cudaStream_t s) {
+  if (!w || !out || !int32_ok(Cout) || !int32_ok(Cin) || Cout_pad < Cout || Cin_pad < Cin || Cout_pad > INT32_MAX || Cin_pad > INT32_MAX)
+    return invalid("hv_pack_conv3x3", "non-NULL pointers, 1 <= Cout <= Cout_pad and 1 <= Cin <= Cin_pad within int32");
+  const int sms = device_sms();
+  if (!sms) return HV_ERR_CUDA;
+  const long long total = Cout_pad * 9 * Cin_pad;
+  pack_conv3x3_kernel<__half><<<blocks_for(total, sms), kThreads, 0, s>>>(w, out, total, static_cast<int>(Cout), static_cast<int>(Cin),
+                                                                           static_cast<int>(Cin_pad));
+  return cuda_status(cudaGetLastError(), "hv_pack_conv3x3");
 }
-cudaError_t launch_pack_conv3x3(const __half* w, __half* out, int Cout, int Cin, int Cout_pad, int Cin_pad, int num_sms, cudaStream_t s) {
-  const long long total = static_cast<long long>(Cout_pad) * 9 * Cin_pad;
-  pack_conv3x3_kernel<__half><<<blocks_for(total, num_sms), kThreads, 0, s>>>(w, out, total, Cout, Cin, Cin_pad);
-  HV_LAUNCH_CHECK();
-}
-cudaError_t launch_pack_upconv2x2(const __half* w, __half* out, int Cout, int Cin, int num_sms, cudaStream_t s) {
+int op_pack_upconv2x2(const __half* w, __half* out, int64_t Cout, int64_t Cin, cudaStream_t s) {
+  if (!w || !out || !int32_ok(Cout) || !int32_ok(Cin)) return invalid("hv_pack_upconv2x2", "non-NULL pointers, Cout and Cin >= 1 within int32");
+  const int sms = device_sms();
+  if (!sms) return HV_ERR_CUDA;
   const long long total = 16LL * Cout * Cin;
-  pack_upconv2x2_kernel<<<blocks_for(total, num_sms), kThreads, 0, s>>>(w, out, total, Cout, Cin);
-  HV_LAUNCH_CHECK();
+  pack_upconv2x2_kernel<<<blocks_for(total, sms), kThreads, 0, s>>>(w, out, total, static_cast<int>(Cout), static_cast<int>(Cin));
+  return cuda_status(cudaGetLastError(), "hv_pack_upconv2x2");
 }
-cudaError_t launch_pack_geglu(const __half* w, __half* out, int rows, int K, int num_sms, cudaStream_t s) {
-  const long long total = static_cast<long long>(rows) * K;
-  pack_geglu_kernel<<<blocks_for(total, num_sms), kThreads, 0, s>>>(w, out, total, rows, K);
-  HV_LAUNCH_CHECK();
+// rows come in blocks of 256 = [128 hidden | 128 gate]
+int op_pack_geglu(const __half* w, __half* out, int64_t rows, int64_t K, cudaStream_t s) {
+  if (!w || !out || !int32_ok(rows) || (rows % 256) || !int32_ok(K))
+    return invalid("hv_pack_geglu", "non-NULL pointers, rows a positive multiple of 256 and K >= 1 within int32");
+  const int sms = device_sms();
+  if (!sms) return HV_ERR_CUDA;
+  const long long total = rows * K;
+  pack_geglu_kernel<<<blocks_for(total, sms), kThreads, 0, s>>>(w, out, total, static_cast<int>(rows), static_cast<int>(K));
+  return cuda_status(cudaGetLastError(), "hv_pack_geglu");
 }
-cudaError_t launch_pack_heads(const __half* w, __half* out, int heads, int d, int dpad, int K, int num_sms, cudaStream_t s) {
+int op_pack_heads(const __half* w, __half* out, int heads, int d, int dpad, int64_t K, cudaStream_t s) {
+  if (!w || !out || heads < 1 || d < 1 || dpad < d || !int32_ok(K) || static_cast<int64_t>(heads) * dpad > INT32_MAX)
+    return invalid("hv_pack_heads", "non-NULL pointers, heads, d, K >= 1, dpad >= d, heads*dpad and K within int32");
+  const int sms = device_sms();
+  if (!sms) return HV_ERR_CUDA;
   const long long total = static_cast<long long>(heads) * dpad * K;
-  pack_heads_kernel<<<blocks_for(total, num_sms), kThreads, 0, s>>>(w, out, total, d, dpad, K);
-  HV_LAUNCH_CHECK();
+  pack_heads_kernel<<<blocks_for(total, sms), kThreads, 0, s>>>(w, out, total, d, dpad, static_cast<int>(K));
+  return cuda_status(cudaGetLastError(), "hv_pack_heads");
 }
-cudaError_t launch_dbg_gemm(const __half* a, long long lda, const __half* w, float* out, int M, int N, int K, cudaStream_t s) {
-  const long long total = static_cast<long long>(M) * N;
-  dbg_gemm_kernel<<<static_cast<unsigned>((total + kThreads - 1) / kThreads), kThreads, 0, s>>>(a, lda, w, out, M, N, K);
-  HV_LAUNCH_CHECK();
+int op_dbg_gemm(const __half* a, int64_t lda, const __half* w, float* out, int64_t M, int64_t N, int64_t K, cudaStream_t s) {
+  if (!a || !w || !out || !int32_ok(M) || !int32_ok(N) || !int32_ok(K) || M * N > INT32_MAX)
+    return invalid("hv_dbg_gemm", "non-NULL pointers, M, N, K >= 1, M*N within int32");
+  const long long total = M * N;
+  dbg_gemm_kernel<<<static_cast<unsigned>((total + kThreads - 1) / kThreads), kThreads, 0, s>>>(a, lda, w, out, static_cast<int>(M), static_cast<int>(N),
+                                                                                              static_cast<int>(K));
+  return cuda_status(cudaGetLastError(), "hv_dbg_gemm");
 }
 
 }  // namespace hv

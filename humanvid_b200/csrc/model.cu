@@ -1,6 +1,6 @@
 // Network runtime behind include/hv_b200.h: weight ingestion under the reference's state_dict keys, packing into
 // kernel layouts, a stack-allocated activation workspace, and the forwards (UNet3DConditionModel, PoseGuider,
-// CameraPoseEncoder, AutoencoderKL encode / decode, CLIPVisionModelWithProjection) expressed as sequences of the operators in ops.h / kernels.h.
+// CameraPoseEncoder, AutoencoderKL encode / decode, CLIPVisionModelWithProjection) expressed as sequences of the operators in ops.h.
 //
 // Activations are channels-last fp16 (N = B*F frames, H, W, C) == a [tokens][C] matrix, so the reference's
 // "b c f h w -> (b f) c h w", "(bf) c h w -> (bf) (hw) c" and "(b f) d c -> (b d) f c" rearranges never touch memory:
@@ -17,10 +17,7 @@
 #include <vector>
 
 #include "../../include/hv_b200.h"
-#include "gemm.cuh"
-#include "kernels.h"
 #include "ops.h"
-#include "tma.h"
 
 namespace hv {
 
@@ -36,6 +33,7 @@ struct Err {
   va_end(ap);
   throw Err{code, buf};
 }
+// ck: a CUDA runtime call (copies, memsets, events); ckop: an operator of ops.h
 static void ck(cudaError_t e, const char* what) {
   if (e != cudaSuccess) fail(HV_ERR_CUDA, "%s: %s", what, cudaGetErrorString(e));
 }
@@ -182,7 +180,6 @@ struct hv_model {
   std::unordered_map<std::string, Raw> raw;
   std::vector<void*> owned;  // cudaMalloc'ed blocks (weights, banks)
   bool finalized = false;
-  int sms = 0;
   cudaStream_t st = nullptr;
   Arena ar;
   void* private_ws = nullptr;
@@ -354,7 +351,7 @@ struct hv_model {
     c.w.rows = c.cout_pad;
     c.w.cols = 9LL * c.cin_pad;
     c.w.p = dmalloc(c.w.rows * c.w.cols);
-    ck(launch_pack_conv3x3(r.p, c.w.p, cout, cin, c.cout_pad, c.cin_pad, sms, st), "pack conv3x3");
+    ckop(op_pack_conv3x3(r.p, c.w.p, cout, cin, c.cout_pad, c.cin_pad, st), "pack conv3x3");
     c.bias = vec(pfx + ".bias", cout, c.cout_pad);
     return c;
   }
@@ -368,7 +365,7 @@ struct hv_model {
     c.w.rows = 4LL * cout;
     c.w.cols = 4LL * cin;
     c.w.p = dmalloc(c.w.rows * c.w.cols);
-    ck(launch_pack_upconv2x2(r.p, c.w.p, cout, cin, sms, st), "pack upconv2x2");
+    ckop(op_pack_upconv2x2(r.p, c.w.p, cout, cin, st), "pack upconv2x2");
     c.bias = vec(pfx + ".bias", cout);
     return c;
   }
@@ -387,9 +384,9 @@ struct hv_model {
     if ((4 * C) % 128) fail(HV_ERR_INVALID, "GEGLU inner dim %d must be a multiple of 128", 4 * C);
     Lin l;
     l.w = Mat{dmalloc(8LL * C * C), 8LL * C, C};
-    ck(launch_pack_geglu(w.p, l.w.p, 8 * C, C, sms, st), "pack geglu");
+    ckop(op_pack_geglu(w.p, l.w.p, 8 * C, C, st), "pack geglu");
     l.bias = dmalloc(8LL * C);
-    ck(launch_pack_geglu(b.p, l.bias, 8 * C, 1, sms, st), "pack geglu bias");
+    ckop(op_pack_geglu(b.p, l.bias, 8 * C, 1, st), "pack geglu bias");
     l.geglu = true;
     return l;
   }
@@ -424,7 +421,7 @@ struct hv_model {
     const int64_t rows = static_cast<int64_t>(heads) * dpad;
     __half* p = dmalloc(static_cast<int64_t>(keys.size()) * rows * cols);
     for (size_t i = 0; i < keys.size(); ++i)
-      ck(launch_pack_heads(mat(keys[i], static_cast<int64_t>(heads) * d, cols).p, p + i * rows * cols, heads, d, dpad, cols, sms, st), "pack heads");
+      ckop(op_pack_heads(mat(keys[i], static_cast<int64_t>(heads) * d, cols).p, p + i * rows * cols, heads, d, dpad, cols, st), "pack heads");
     return p;
   }
   // q / k / v / out: key prefixes of the projections; bias: q, k and v have biases (out always has one)
@@ -703,15 +700,15 @@ struct hv_model {
     float* stats = static_cast<float*>(ar.alloc(sizeof(float) * groupnorm_scratch_floats(x.C + C2, x.NF, x.H * x.W, cfg.norm_groups)));
     if (pool_F > 1) {
       launch(3, {CAT_NORM, "groupnorm_pooled", 0, x.rows(), x.C + C2, 0}, [&] {   // statistics + finalize + apply
-        ck(launch_groupnorm_pooled(x.p, x.C, x2 ? x2->p : nullptr, C2, n.g, n.b, out.p, x.NF, x.H * x.W, cfg.norm_groups, n.eps, silu ? 1 : 0, pool_F,
-                                   stats, st),
-           "groupnorm (pooled over frames)");
+        ckop(op_groupnorm_pooled(x.p, x.C, x2 ? x2->p : nullptr, C2, n.g, n.b, out.p, x.NF, x.H * x.W, cfg.norm_groups, n.eps, silu ? 1 : 0, pool_F,
+                                 stats, st),
+             "groupnorm (pooled over frames)");
       });
       return out;
     }
     launch(2, {CAT_NORM, "groupnorm", 0, x.rows(), x.C + C2, 0}, [&] {   // statistics + apply
-      ck(launch_groupnorm(x.p, x.C, x2 ? x2->p : nullptr, C2, n.g, n.b, out.p, x.NF, x.H * x.W, cfg.norm_groups, n.eps, silu ? 1 : 0, stats, st),
-         "groupnorm");
+      ckop(op_groupnorm(x.p, x.C, x2 ? x2->p : nullptr, C2, n.g, n.b, out.p, x.NF, x.H * x.W, cfg.norm_groups, n.eps, silu ? 1 : 0, stats, st),
+           "groupnorm");
     });
     return out;
   }
@@ -722,7 +719,7 @@ struct hv_model {
     Tens t = alloc_act(B * F, H, W, Cpad);
     launch(2, {}, [&] {
       ck(cudaMemsetAsync(t.p, 0, static_cast<size_t>(t.numel()) * 2, st), "memset");
-      ck(launch_ncfhw_to_nhwc(x, t.p, B, C, F, H, W, 0, st, Cpad), "input layout");
+      ckop(op_ncfhw_to_nhwc(x, t.p, B, C, F, H, W, 0, st, Cpad), "input layout");
     });
     return t;
   }
@@ -730,7 +727,7 @@ struct hv_model {
   Tens op_ln(const Tens& x, const Norm& n, const __half* pre_add = nullptr, int64_t rows_per_b = 1, const __half* pe = nullptr, int F = 1) {
     Tens out = alloc_act(x.NF, x.H, x.W, x.C);
     launch(1, {CAT_NORM, "layernorm", 0, x.rows(), x.C, 0}, [&] {
-      ck(launch_layernorm(x.p, n.g, n.b, out.p, x.rows(), x.C, n.eps, pre_add, rows_per_b, nullptr, pe, x.H * x.W, F, st), "layernorm");
+      ckop(op_layernorm(x.p, n.g, n.b, out.p, x.rows(), x.C, n.eps, pre_add, rows_per_b, nullptr, pe, x.H * x.W, F, st), "layernorm");
     });
     return out;
   }
@@ -789,7 +786,7 @@ struct hv_model {
   __half* op_small_linear(const __half* x, const Lin& l, int M, int act_in) {
     __half* out = alloc_h(static_cast<int64_t>(M) * l.w.rows);
     launch(1, {CAT_MISC, "", 2.0 * M * l.w.rows * l.w.cols}, [&] {
-      ck(launch_small_linear(x, l.w.p, l.bias, out, M, static_cast<int>(l.w.rows), static_cast<int>(l.w.cols), act_in, st), "small_linear");
+      ckop(hv::op_small_linear(x, l.w.p, l.bias, out, M, l.w.rows, l.w.cols, act_in, st), "small_linear");
     });
     return out;
   }
@@ -840,21 +837,13 @@ struct hv_model {
     const double flops = 4.0 * L * a.heads * a.d * (static_cast<double>(xn.NF) * L + static_cast<double>(xn.NF - b.nf_nobank) * b.L);
     if (a.dv == a.d) {   // single head, d = 512
       if (b.L > 0) fail(HV_ERR_INVALID, "the d = 512 attention reads no reference bank");
-      launch(1, {CAT_ATTN, "attn_d512", flops, xn.NF, L, a.d}, [&] {
-        cudaError_t e = launch_attention_d512(qk.p, 2 * hp, qk.p + hp, 2 * hp, vt, ldvt, Lp, o.p, C, xn.NF, L, st);
-        if (e != cudaSuccess) fail(HV_ERR_CUDA, "attention d512: %s %s", cudaGetErrorString(e), tma_last_error());
-      });
+      launch(1, {CAT_ATTN, "attn_d512", flops, xn.NF, L, a.d},
+             [&] { ckop(op_attention_d512(qk.p, 2 * hp, qk.p + hp, 2 * hp, vt, ldvt, Lp, o.p, C, xn.NF, L, st), "attention d512"); });
     } else {
       launch(1, {CAT_ATTN, "attn", flops, xn.NF, L, a.d}, [&] {
-        AttnArgs g{};
-        g.q = qk.p; g.k = qk.p + hp; g.vt = vt; g.out = o.p;
-        g.NF = xn.NF; g.L = L; g.heads = a.heads; g.d = a.d; g.dpad = a.dpad;
-        g.ldq = 2 * hp; g.ldk = 2 * hp; g.ldvt = ldvt; g.ldo = C;
-        g.kb = b.k; g.vbt = b.vt; g.Lb = b.L; g.ldkb = hp; g.ldvbt = b.ldvt;
-        g.F = b.F; g.nf_nobank = b.nf_nobank;
-        g.vt_stride = Lp; g.vbt_stride = b.vt_stride;
-        cudaError_t e = launch_attention(g, sms, st);
-        if (e != cudaSuccess) fail(HV_ERR_CUDA, "attention (d = %d): %s %s", a.d, cudaGetErrorString(e), tma_last_error());
+        ckop(op_attention(qk.p, qk.p + hp, vt, o.p, xn.NF, L, a.heads, a.d, 2 * hp, 2 * hp, ldvt, C, b.k, b.vt, b.L, hp, b.ldvt, b.F, b.nf_nobank, Lp,
+                          b.vt_stride, st),
+             "attention");
       });
     }
     op_linear(o, a.out, &res, &out);
@@ -932,7 +921,7 @@ struct hv_model {
     Tens qkv = op_linear(n, a.qkv);
     Tens o = alloc_act(t.NF, t.H, t.W, C);
     launch(1, {CAT_TATTN, "tattn", 4.0 * t.rows() * F * C, t.rows(), F, C},
-           [&] { ck(launch_temporal_attention(qkv.p, o.p, B, F, t.H * t.W, heads, d, st), "temporal attention"); });
+           [&] { ckop(op_temporal_attention(qkv.p, o.p, B, F, t.H * t.W, heads, d, st), "temporal attention"); });
     return op_linear(o, a.out, &t, &out);
   }
   // TemporalTransformerBlock: the temporal attentions, then t = ff(LN(t)) + t
@@ -979,13 +968,13 @@ struct hv_model {
     if ((H % 8) || (W % 8)) fail(HV_ERR_INVALID, "latent size %dx%d must be a multiple of 8 (three stride-2 levels)", H, W);
     // time embedding (unet_3d.py:446-467)
     __half* tsin = alloc_h(static_cast<int64_t>(B) * ch[0]);
-    launch(1, {}, [&] { ck(launch_timestep_embedding(timestep, ts_table, ts_index, tsin, B, ch[0], st), "timestep embedding"); });
+    launch(1, {}, [&] { ckop(op_timestep_embedding(timestep, ts_table, ts_index, tsin, B, ch[0], st), "timestep embedding"); });
     __half* e1 = op_small_linear(tsin, te1, B, HV_ACT_NONE);
     __half* emb = op_small_linear(e1, te2, B, HV_ACT_SILU);
     // conv_in (+ pose_cond_fea as the epilogue residual)
     Tens x0 = padded_input(sample, B, cfg.in_channels, F, H, W, conv_in.cin_pad);
     Tens pc = pose ? alloc_act(NF, H, W, ch[0]) : Tens{};
-    if (pose) launch(1, {}, [&] { ck(launch_ncfhw_to_nhwc(pose, pc.p, B, ch[0], F, H, W, 0, st), "pose layout"); });
+    if (pose) launch(1, {}, [&] { ckop(op_ncfhw_to_nhwc(pose, pc.p, B, ch[0], F, H, W, 0, st), "pose layout"); });
     Tens h = op_conv3(x0, conv_in, 1, pose ? &pc : nullptr);
     tap("conv_in", h);
     // layer j of stage s (skip: the down-path tensor an up-path resnet concatenates)
@@ -1022,12 +1011,12 @@ struct hv_model {
       }
     }
     if (cfg.kind == HV_KIND_UNET2D_REF) {   // no post-process: the forward's value is the last up block's output (B, C0, h, w)
-      if (outp != nullptr) launch(1, {}, [&] { ck(launch_nhwc_to_ncfhw(h.p, h.C, outp, B, ch[0], F, H, W, st), "hidden layout"); });
+      if (outp != nullptr) launch(1, {}, [&] { ckop(op_nhwc_to_ncfhw(h.p, h.C, outp, B, ch[0], F, H, W, st), "hidden layout"); });
       return;
     }
     Tens hn = op_gn(h, nullptr, norm_out, true, gn_pool(F));
     Tens y = op_conv3(hn, conv_out);
-    launch(1, {}, [&] { ck(launch_nhwc_to_ncfhw(y.p, y.C, outp, B, cfg.out_channels, F, H, W, st), "output layout"); });
+    launch(1, {}, [&] { ckop(op_nhwc_to_ncfhw(y.p, y.C, outp, B, cfg.out_channels, F, H, W, st), "output layout"); });
   }
 
   void pose_guider_forward(const __half* cond, __half* outp, int B, int F, int H, int W) {
@@ -1038,14 +1027,14 @@ struct hv_model {
       // conv_in (3 -> 16) straight from the (B, 3, F, H, W) image: no layout pass, 16-channel output
       h = alloc_act(NF, H, W, pg_in.cout);
       launch(1, {CAT_CONV, "pg_conv_in", 2.0 * h.rows() * pg_in.cout * 9.0 * pg_in.cin, h.rows(), pg_in.cout, 9LL * pg_in.cin},
-             [&] { ck(launch_pg_conv_in(cond, pg_in.w, pg_in.bias, h.p, B, F, H, W, HV_ACT_SILU, sms, st), "pose conv_in"); });
+             [&] { ckop(op_pose_conv_in(cond, pg_in.w, pg_in.bias, h.p, B, F, H, W, HV_ACT_SILU, st), "pose conv_in"); });
     } else {
       Tens x0 = alloc_act(NF, H, W, cfg.pg_cond_channels);
       h = alloc_act(NF, H, W, pg_convs[0].cin_pad);
       launch(3, {}, [&] {
-        ck(launch_ncfhw_to_nhwc(cond, x0.p, B, cfg.pg_cond_channels, F, H, W, 0, st), "pose image layout");
+        ckop(op_ncfhw_to_nhwc(cond, x0.p, B, cfg.pg_cond_channels, F, H, W, 0, st), "pose image layout");
         ck(cudaMemsetAsync(h.p, 0, static_cast<size_t>(h.numel()) * 2, st), "memset");
-        ck(launch_conv3x3_direct_padded(x0.p, pg_in.w, pg_in.bias, h.p, NF, H, W, pg_in.cin, pg_in.cout, h.C, HV_ACT_SILU, sms, st), "pose conv_in");
+        ckop(op_conv3x3_direct(x0.p, pg_in.w, pg_in.bias, h.p, NF, H, W, pg_in.cin, pg_in.cout, 1, HV_ACT_SILU, nullptr, h.C, st), "pose conv_in");
       });
     }
     for (size_t i = 0; i < pg_convs.size(); ++i) {
@@ -1059,7 +1048,7 @@ struct hv_model {
         Tens out = alloc_act(NF, Ho, Wo, ld);
         if (ld > c.cout) launch(1, {}, [&] { ck(cudaMemsetAsync(out.p, 0, static_cast<size_t>(out.numel()) * 2, st), "memset"); });
         launch(1, {CAT_CONV, pg_strides[i] == 1 ? "smallconv" : "smallconv_s2", 2.0 * out.rows() * c.cout * 9.0 * c.cin, out.rows(), c.cout, 9LL * c.cin},
-               [&] { ck(launch_smallconv(h.p, c.w.p, c.bias, out.p, NF, h.H, h.W, c.cin, c.cout, pg_strides[i], ld, HV_ACT_SILU, st), "pose small conv"); });
+               [&] { ckop(op_conv3x3_small(h.p, c.w.p, c.bias, out.p, ld, NF, h.H, h.W, c.cin, c.cout, pg_strides[i], HV_ACT_SILU, st), "pose small conv"); });
         h = out;
         continue;
       }
@@ -1067,7 +1056,7 @@ struct hv_model {
       // the next conv expects cin_pad channels: cout_pad of this conv equals it by construction (both round to 64)
       if (!last && h.C != pg_convs[i + 1].cin_pad) fail(HV_ERR_INVALID, "pose guider channel padding mismatch at conv %zu", i);
     }
-    launch(1, {}, [&] { ck(launch_nhwc_to_ncfhw(h.p, h.C, outp, B, cfg.pg_out_channels, F, h.H, h.W, st), "pose output layout"); });
+    launch(1, {}, [&] { ckop(op_nhwc_to_ncfhw(h.p, h.C, outp, B, cfg.pg_out_channels, F, h.H, h.W, st), "pose output layout"); });
   }
 
   void camera_forward(const __half* plucker, __half* outp, int B, int F, int H, int W, const float* rays_K = nullptr, const float* rays_c2w = nullptr) {
@@ -1078,9 +1067,9 @@ struct hv_model {
     if (rays_K != nullptr && cin0 != 6) fail(HV_ERR_INVALID, "the Plucker producer makes 6 channels, encoder expects %d", cin0);
     launch(1, {}, [&] {
       if (rays_K != nullptr)   // SURVEY 8f-3: Plucker embedding generated in place of the unshuffle's gather
-        ck(launch_plucker_unshuffle(rays_K, rays_c2w, u.p, NF, H, W, r, sms, st), "plucker unshuffle");
+        ckop(op_plucker_unshuffle(rays_K, rays_c2w, u.p, NF, H, W, r, st), "plucker unshuffle");
       else
-        ck(launch_pixel_unshuffle(plucker, u.p, B, cin0, F, H, W, r, sms, st), "pixel unshuffle");
+        ckop(op_pixel_unshuffle(plucker, u.p, B, cin0, F, H, W, r, st), "pixel unshuffle");
     });
     Tens x = op_conv3(u, cam_in);
     for (int j = 0; j < cfg.cam_nums_rb; ++j) {
@@ -1090,7 +1079,7 @@ struct hv_model {
       x = tblock_fwd(cam_att[j], x, B, F);   // over the frame axis
     }
     Tens z = op_linear(x, cam_zero);
-    launch(1, {}, [&] { ck(launch_nhwc_to_ncfhw(z.p, z.C, outp, NF, C, 1, z.H, z.W, st), "camera output layout"); });
+    launch(1, {}, [&] { ckop(op_nhwc_to_ncfhw(z.p, z.C, outp, NF, C, 1, z.H, z.W, st), "camera output layout"); });
   }
 
   // ================================================================== AutoencoderKL
@@ -1118,7 +1107,7 @@ struct hv_model {
     Tens hn = op_gn(h, nullptr, enc.norm_out, true);
     Tens y = op_conv3(hn, enc.conv_out);
     Tens m = op_linear(y, quant);   // quant_conv (1x1)
-    launch(1, {}, [&] { ck(launch_nhwc_to_ncfhw(m.p, m.C, moments, N, m.C, 1, m.H, m.W, st), "moments layout"); });
+    launch(1, {}, [&] { ckop(op_nhwc_to_ncfhw(m.p, m.C, moments, N, m.C, 1, m.H, m.W, st), "moments layout"); });
   }
   void vae_decode(const __half* z, __half* outp, int N, int H, int W) {
     if (N <= 0 || H <= 0 || W <= 0) fail(HV_ERR_INVALID, "AutoencoderKL.decode: N = %d latents of %dx%d must all be positive", N, H, W);
@@ -1132,7 +1121,7 @@ struct hv_model {
     }
     Tens hn = op_gn(h, nullptr, dec.norm_out, true);
     Tens y = op_conv3(hn, dec.conv_out);
-    launch(1, {}, [&] { ck(launch_nhwc_to_ncfhw(y.p, y.C, outp, N, cfg.out_channels, 1, y.H, y.W, st), "image output layout"); });
+    launch(1, {}, [&] { ckop(op_nhwc_to_ncfhw(y.p, y.C, outp, N, cfg.out_channels, 1, y.H, y.W, st), "image output layout"); });
   }
 
   // ================================================================== CLIPVisionModelWithProjection
@@ -1159,12 +1148,12 @@ struct hv_model {
     const int C = cfg.clip_hidden_size, p = cfg.clip_patch_size, np = (S / p) * (S / p), L = np + 1, Kpad = clip_kpad();
     // patch embedding: the stride-p conv as patchify + GEMM
     Tens prow = alloc_act(B, 1, np, Kpad);
-    launch(1, {}, [&] { ck(launch_clip_patchify(pix, prow.p, B, 3, S, p, Kpad, sms, st), "patchify"); });
+    launch(1, {}, [&] { ckop(op_clip_patchify(pix, prow.p, B, 3, S, p, Kpad, st), "patchify"); });
     Tens pe = op_linear(prow, clip_patch);
     // [class_embedding ; patches] + position_embedding -> pre_layrnorm: the residual stream (B images x L tokens)
     Tens x = alloc_act(B, 1, L, C);
     launch(1, {CAT_NORM, "clip_embed_ln", 0, x.rows(), C, 0},
-           [&] { ck(launch_clip_embed_ln(pe.p, clip_cls, clip_pos, clip_pre.g, clip_pre.b, x.p, x.rows(), L, C, clip_pre.eps, st), "embeddings + pre_layrnorm"); });
+           [&] { ckop(op_clip_embed_ln(pe.p, clip_cls, clip_pos, clip_pre.g, clip_pre.b, x.p, x.rows(), L, C, clip_pre.eps, st), "embeddings + pre_layrnorm"); });
     for (size_t i = 0; i < clip_layers.size(); ++i) {
       const bool last = i + 1 == clip_layers.size();
       __half* dst = last && lhs != nullptr ? lhs : x.p;   // the stream is updated in place; the last layer writes the caller's last_hidden_state
@@ -1180,7 +1169,7 @@ struct hv_model {
     Tens pooled = op_ln(cls, clip_post);
     const int P = static_cast<int>(clip_proj.rows);
     launch(1, {CAT_MISC, "", 2.0 * B * P * C},
-           [&] { ck(launch_small_linear(pooled.p, clip_proj.p, nullptr, embeds, B, P, C, HV_ACT_NONE, st), "visual_projection"); });
+           [&] { ckop(hv::op_small_linear(pooled.p, clip_proj.p, nullptr, embeds, B, P, C, HV_ACT_NONE, st), "visual_projection"); });
   }
 };
 
@@ -1257,11 +1246,9 @@ int hv_create(const hv_config* cfg, hv_handle* out) {
   if (!cfg || !out) return HV_ERR_INVALID;
   hv_model* m = nullptr;
   try {
-    const int sms = device_sms();
-    if (!sms) fail(HV_ERR_CUDA, "%s", last_error());
+    if (!device_sms()) fail(HV_ERR_CUDA, "%s", last_error());
     m = new hv_model();
     m->cfg = *cfg;
-    m->sms = sms;
     if (cfg->kind < 0 || cfg->kind > HV_KIND_CLIP_VISION) fail(HV_ERR_INVALID, "unknown kind %d", cfg->kind);
     if (cfg->kind == HV_KIND_UNET2D_REF && cfg->use_motion_module) fail(HV_ERR_INVALID, "the reference (writer) UNet has no motion modules");
     *out = m;

@@ -5,6 +5,7 @@
 #include <stdint.h>
 #include <stdlib.h>
 
+#include "ops.h"
 #include "ptx.cuh"
 
 namespace hv {
@@ -441,14 +442,19 @@ __global__ void __launch_bounds__(128) clip_embed_ln_kernel(const __half* __rest
 
 }  // namespace
 
-cudaError_t launch_clip_embed_ln(const __half* patch, const __half* cls, const __half* pos, const __half* gamma, const __half* beta, __half* out,
-                                 long long rows, int L, int C, float eps, cudaStream_t stream) {
-  if (C % 8 || C / 8 > 256 || L < 1 || rows <= 0 || rows % L || rows > 0x7fffffffLL) return cudaErrorInvalidValue;
-  clip_embed_ln_kernel<<<static_cast<unsigned>(rows), 128, 0, stream>>>(patch, cls, pos, gamma, beta, out, L, C, eps);
-  return cudaGetLastError();
+int op_clip_embed_ln(const __half* patch, const __half* cls, const __half* pos, const __half* gamma, const __half* beta, __half* out, int64_t rows,
+                     int64_t L, int64_t C, float eps, cudaStream_t stream) {
+  if (!patch || !cls || !pos || !gamma || !beta || !out || !aligned16(patch) || !aligned16(cls) || !aligned16(pos) || !aligned16(gamma) ||
+      !aligned16(beta) || !aligned16(out) || C % 8 || C / 8 > 256 || L < 1 || rows <= 0 || rows % L || rows > INT32_MAX) {
+    set_error("clip_embed_ln: bad arguments rows=%lld L=%lld C=%lld (16-byte aligned tensors, C a multiple of 8 <= 2048, L divides rows)",
+              (long long)rows, (long long)L, (long long)C);
+    return HV_ERR_INVALID;
+  }
+  clip_embed_ln_kernel<<<static_cast<unsigned>(rows), 128, 0, stream>>>(patch, cls, pos, gamma, beta, out, static_cast<int>(L), static_cast<int>(C), eps);
+  return cuda_status(cudaGetLastError(), "clip_embed_ln");
 }
 
-// scratch floats needed by launch_groupnorm: final {mean, rstd} + per-slab partials
+// scratch floats needed by op_groupnorm: final {mean, rstd} + per-slab partials
 // The split of a frame's rows into slabs (= the order its statistics are summed in) depends on HW only, never on the number of frames in
 // the batch: a forward of one CFG half (a unit of the multi-GPU split) is then bitwise equal to that half of a CFG batch.
 // (Measured and rejected: normalising ~56 MB chunks of frames at a time so that the apply pass re-reads from L2 what the statistics pass
@@ -471,74 +477,96 @@ size_t groupnorm_scratch_floats(int C, int NF, int HW, int groups) {
   return static_cast<size_t>(2) * NF * groups * (1 + sl);
 }
 
-bool groupnorm_shape_ok(int C1, int C2, int HW, int groups) {
-  const int C = C1 + C2;
-  if (groups <= 0 || C % 8 || C1 % 8 || C % groups || ((C / groups) & 1) || groups > 32 * 8) return false;
-  const int vecs = C / 8;
-  if (vecs > 1024) return false;
-  int threads, slabs, rows_per_block;
-  gn_plan(C, HW, &threads, &slabs, &rows_per_block);
-  return threads >= groups && threads >= 32;
+// The arguments both GroupNorms can run: F = frames per item (1 for op_groupnorm).  The kernels load X, X2, gamma, beta and out 16 bytes
+// at a time and stats as float2; NF is the grid's y dimension.
+static int check_groupnorm(const char* op, const __half* X, int64_t C1, const __half* X2, int64_t C2, const __half* gamma, const __half* beta,
+                           const __half* out, int64_t NF, int64_t HW, int groups, int64_t F, const float* stats) {
+  bool ok = X && gamma && beta && out && stats && (C2 == 0 || X2) && C1 > 0 && C2 >= 0 && C1 + C2 <= 8192 && NF > 0 && HW > 0 && HW <= INT32_MAX &&
+            F > 0 && NF % F == 0 && NF <= 65535 && aligned16(X) && (C2 == 0 || aligned16(X2)) && aligned16(gamma) && aligned16(beta) &&
+            aligned16(out) && (reinterpret_cast<uintptr_t>(stats) & 7) == 0;
+  const int C = static_cast<int>(C1 + C2);
+  // the channel layouts the kernels run; gn_plan divides by C / 8, so it comes after C % 8 == 0 (and C1 > 0)
+  ok = ok && groups > 0 && C % 8 == 0 && C1 % 8 == 0 && C % groups == 0 && ((C / groups) & 1) == 0 && groups <= 32 * 8;
+  if (ok) {
+    int threads, slabs, rows_per_block;
+    gn_plan(C, static_cast<int>(HW), &threads, &slabs, &rows_per_block);
+    ok = threads >= groups && threads >= 32;
+  }
+  if (!ok)
+    set_error("%s: bad arguments C1=%lld C2=%lld NF=%lld HW=%lld groups=%d frames_per_item=%lld (NF %% F == 0, NF <= 65535, 16-byte aligned "
+              "tensors, 8-byte aligned stats, C1 and C1 + C2 multiples of 8, C1 + C2 <= 8192, C / groups even, groups <= 256)", op, (long long)C1,
+              (long long)C2, (long long)NF, (long long)HW, groups, (long long)F);
+  return ok ? HV_OK : HV_ERR_INVALID;
 }
 
-cudaError_t launch_groupnorm(const __half* x1, int C1, const __half* x2, int C2, const __half* gamma, const __half* beta,
-                             __half* out, int NF, int HW, int groups, float eps, int silu, float* stats, cudaStream_t stream) {
-  const int C = C1 + C2;
-  if (!groupnorm_shape_ok(C1, C2, HW, groups)) return cudaErrorInvalidValue;
+int op_groupnorm(const __half* x1, int64_t C1, const __half* x2, int64_t C2, const __half* gamma, const __half* beta, __half* out, int64_t NF,
+                 int64_t HW, int groups, float eps, int silu, float* stats, cudaStream_t stream) {
+  if (int rc = check_groupnorm("hv_op_groupnorm", x1, C1, x2, C2, gamma, beta, out, NF, HW, groups, 1, stats)) return rc;
+  const int C = static_cast<int>(C1 + C2);
   int threads, slabs, rows_per_block;
-  gn_plan(C, HW, &threads, &slabs, &rows_per_block);
+  gn_plan(C, static_cast<int>(HW), &threads, &slabs, &rows_per_block);
   float* partial = stats + static_cast<size_t>(2) * NF * groups;
-  gn_stats_kernel<<<dim3(slabs, NF), threads, threads * 8 * sizeof(float), stream>>>(x1, C1, x2, C2, HW, groups, rows_per_block, partial);
+  gn_stats_kernel<<<dim3(slabs, static_cast<unsigned>(NF)), threads, threads * 8 * sizeof(float), stream>>>(x1, static_cast<int>(C1), x2, static_cast<int>(C2),
+                                                                                                          static_cast<int>(HW), groups, rows_per_block, partial);
   // (the {mean, rstd} finalize is folded into the apply kernel: one launch less per GroupNorm, 83 per forward)
-  gn_apply_kernel<<<dim3(slabs, NF), threads, groups * sizeof(float2), stream>>>(x1, C1, x2, C2, gamma, beta, out, HW, groups, rows_per_block, silu, partial,
-                                                                                 slabs, 1.f / (static_cast<float>(HW) * (C / groups)), eps);
-  return cudaGetLastError();
+  gn_apply_kernel<<<dim3(slabs, static_cast<unsigned>(NF)), threads, groups * sizeof(float2), stream>>>(
+      x1, static_cast<int>(C1), x2, static_cast<int>(C2), gamma, beta, out, static_cast<int>(HW), groups, rows_per_block, silu, partial, slabs,
+      1.f / (static_cast<float>(static_cast<int>(HW)) * (C / groups)), eps);
+  return cuda_status(cudaGetLastError(), "hv_op_groupnorm");
 }
 
-// Statistics pooled over the F frames of each batch item (nn.GroupNorm on a (b, c, f, h, w) tensor).  Same scratch as launch_groupnorm:
+// Statistics pooled over the F frames of each batch item (nn.GroupNorm on a (b, c, f, h, w) tensor).  Same scratch as op_groupnorm:
 // the per-frame partials at the same offset, and the items' {mean, rstd} in the first 2 * (NF / F) * groups floats.  At F = 1 this is
-// launch_groupnorm itself.
-cudaError_t launch_groupnorm_pooled(const __half* x1, int C1, const __half* x2, int C2, const __half* gamma, const __half* beta,
-                                    __half* out, int NF, int HW, int groups, float eps, int silu, int F, float* stats, cudaStream_t stream) {
-  if (F <= 0 || NF % F) return cudaErrorInvalidValue;
-  if (F == 1) return launch_groupnorm(x1, C1, x2, C2, gamma, beta, out, NF, HW, groups, eps, silu, stats, stream);
-  const int C = C1 + C2;
-  if (!groupnorm_shape_ok(C1, C2, HW, groups)) return cudaErrorInvalidValue;
+// op_groupnorm itself.
+int op_groupnorm_pooled(const __half* x1, int64_t C1, const __half* x2, int64_t C2, const __half* gamma, const __half* beta, __half* out,
+                        int64_t NF, int64_t HW, int groups, float eps, int silu, int64_t F, float* stats, cudaStream_t stream) {
+  if (int rc = check_groupnorm("hv_op_groupnorm_pooled", x1, C1, x2, C2, gamma, beta, out, NF, HW, groups, F, stats)) return rc;
+  if (C2 == 0) x2 = nullptr;
+  if (F == 1) return op_groupnorm(x1, C1, x2, C2, gamma, beta, out, NF, HW, groups, eps, silu, stats, stream);
+  const int C = static_cast<int>(C1 + C2), Fi = static_cast<int>(F), HWi = static_cast<int>(HW);
   int threads, slabs, rows_per_block;
-  gn_plan(C, HW, &threads, &slabs, &rows_per_block);
+  gn_plan(C, HWi, &threads, &slabs, &rows_per_block);
   float2* stat = reinterpret_cast<float2*>(stats);
   float* partial = stats + static_cast<size_t>(2) * NF * groups;
-  gn_stats_pooled_kernel<<<dim3(slabs, NF), threads, threads * 8 * sizeof(float), stream>>>(x1, C1, x2, C2, HW, groups, rows_per_block, partial, F);
-  gn_finalize_pooled_kernel<<<dim3(groups, NF / F), kGnFinalizeThreads, 0, stream>>>(x1, C1, x2, C2, HW, groups, partial, slabs, F,
-                                                                                      1.f / (static_cast<float>(F) * HW * (C / groups)), eps, stat);
-  gn_apply_pooled_kernel<<<dim3(slabs, NF), threads, 0, stream>>>(x1, C1, x2, C2, gamma, beta, out, HW, groups, rows_per_block, silu, stat, F);
-  return cudaGetLastError();
+  const dim3 grid(slabs, static_cast<unsigned>(NF));
+  gn_stats_pooled_kernel<<<grid, threads, threads * 8 * sizeof(float), stream>>>(x1, static_cast<int>(C1), x2, static_cast<int>(C2), HWi, groups,
+                                                                                 rows_per_block, partial, Fi);
+  gn_finalize_pooled_kernel<<<dim3(groups, static_cast<unsigned>(NF / F)), kGnFinalizeThreads, 0, stream>>>(
+      x1, static_cast<int>(C1), x2, static_cast<int>(C2), HWi, groups, partial, slabs, Fi, 1.f / (static_cast<float>(Fi) * HWi * (C / groups)), eps, stat);
+  gn_apply_pooled_kernel<<<grid, threads, 0, stream>>>(x1, static_cast<int>(C1), x2, static_cast<int>(C2), gamma, beta, out, HWi, groups,
+                                                       rows_per_block, silu, stat, Fi);
+  return cuda_status(cudaGetLastError(), "hv_op_groupnorm_pooled");
 }
 
-cudaError_t launch_layernorm(const __half* x, const __half* gamma, const __half* beta, __half* out, long long rows, int C, float eps,
-                             const __half* pre_add, long long rows_per_group, __half* x_out, const __half* pe, int hw, int F,
-                             cudaStream_t stream) {
-  if (C % 8) return cudaErrorInvalidValue;
-  const int vecs = C / 8;
-  if (vecs > 160) return cudaErrorInvalidValue;
+// The kernel holds up to 160 vectors of 8 per row (C <= 1280) and loads x, pre_add, gamma, beta and pe and stores out and x_out 16 bytes at a time.
+int op_layernorm(const __half* x, const __half* gamma, const __half* beta, __half* out, int64_t rows, int64_t C, float eps, const __half* pre_add,
+                 int64_t rows_per_group, __half* x_out, const __half* pe, int64_t hw, int64_t F, cudaStream_t stream) {
+  if (!x || !gamma || !beta || !out || !aligned16(x) || !aligned16(gamma) || !aligned16(beta) || !aligned16(out) || !aligned16(pre_add) ||
+      !aligned16(x_out) || !aligned16(pe) || rows < 1 || C < 8 || C > 1280 || C % 8 || hw > INT32_MAX || F > INT32_MAX) {
+    set_error("hv_op_layernorm: bad arguments rows=%lld C=%lld hw=%lld F=%lld (non-NULL, 16-byte aligned tensors, rows >= 1, C a multiple of 8 "
+              "<= 1280, hw and F <= INT32_MAX)", (long long)rows, (long long)C, (long long)hw, (long long)F);
+    return HV_ERR_INVALID;
+  }
+  const int vecs = static_cast<int>(C / 8);
   if (rows_per_group <= 0) rows_per_group = 1;
   if (hw <= 0) hw = 1;
   if (F <= 0) F = 1;
   const int lpr = vecs <= 40 ? 8 : (vecs <= 80 ? 16 : 32);
   const int wpb = 8;
   const long long warps = (rows + (32 / lpr) - 1) / (32 / lpr);
-  static int sms = 0;
-  if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); }
+  const int sms = device_sms();
+  if (!sms) return HV_ERR_CUDA;
   long long blocks = (warps + wpb - 1) / wpb;
   if (blocks > 8LL * sms) blocks = 8LL * sms;   // persistent grid: 8 blocks per SM
   const unsigned grid = static_cast<unsigned>(blocks);
+  const int Ci = static_cast<int>(C), hwi = static_cast<int>(hw), Fi = static_cast<int>(F);
   if (lpr == 8)
-    layernorm_kernel<8><<<grid, wpb * 32, 0, stream>>>(x, gamma, beta, out, rows, C, eps, pre_add, rows_per_group, x_out, pe, hw, F);
+    layernorm_kernel<8><<<grid, wpb * 32, 0, stream>>>(x, gamma, beta, out, rows, Ci, eps, pre_add, rows_per_group, x_out, pe, hwi, Fi);
   else if (lpr == 16)
-    layernorm_kernel<16><<<grid, wpb * 32, 0, stream>>>(x, gamma, beta, out, rows, C, eps, pre_add, rows_per_group, x_out, pe, hw, F);
+    layernorm_kernel<16><<<grid, wpb * 32, 0, stream>>>(x, gamma, beta, out, rows, Ci, eps, pre_add, rows_per_group, x_out, pe, hwi, Fi);
   else
-    layernorm_kernel<32><<<grid, wpb * 32, 0, stream>>>(x, gamma, beta, out, rows, C, eps, pre_add, rows_per_group, x_out, pe, hw, F);
-  return cudaGetLastError();
+    layernorm_kernel<32><<<grid, wpb * 32, 0, stream>>>(x, gamma, beta, out, rows, Ci, eps, pre_add, rows_per_group, x_out, pe, hwi, Fi);
+  return cuda_status(cudaGetLastError(), "hv_op_layernorm");
 }
 
 }  // namespace hv

@@ -6,7 +6,6 @@
 #include <stdlib.h>
 
 #include "gemm.cuh"
-#include "kernels.h"
 #include "tma.h"
 
 namespace hv {
@@ -23,7 +22,8 @@ void set_error(const char* fmt, ...) {
   va_end(ap);
 }
 const char* last_error() { return g_msg; }
-int cuda_fail(cudaError_t e, const char* what) {
+int cuda_status(cudaError_t e, const char* what) {
+  if (e == cudaSuccess) return HV_OK;
   set_error("%s: %s", what, cudaGetErrorString(e));
   return HV_ERR_CUDA;
 }
@@ -120,12 +120,12 @@ static GemmProblem linear_problem(int64_t M, int64_t N, int64_t K, bool geglu, i
 }
 
 int plan_linear(int64_t M, int64_t N, int64_t K, bool geglu, int* block_n, int* bst_stages, int* grid) {
-  const int sms = device_sms();
-  if (!sms) return HV_ERR_CUDA;
   if (M <= 0 || N <= 0 || K <= 0 || M > INT32_MAX || N > INT32_MAX || K > INT32_MAX) {
     set_error("hv_dbg_gemm_plan: bad shape M=%lld N=%lld K=%lld", (long long)M, (long long)N, (long long)K);
     return HV_ERR_INVALID;
   }
+  const int sms = device_sms();
+  if (!sms) return HV_ERR_CUDA;
   int bn;
   const GemmProblem p = linear_problem(M, N, K, geglu, sms, &bn);
   GemmPlan plan;
@@ -139,11 +139,20 @@ int plan_linear(int64_t M, int64_t N, int64_t K, bool geglu, int* block_n, int* 
   return HV_OK;
 }
 
+// The launch of a problem the caller has checked and mapped; HV_ERR_INVALID when no plan fits it.
+static int run_gemm(const char* op, const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const CUtensorMap& out,
+                    const CUtensorMap& res, const GemmProblem& p, const GemmEpilogue& e, int bn, int sms, cudaStream_t stream) {
+  GemmPlan plan;
+  if (!plan_gemm(p, bn, sms, &plan)) {
+    set_error("%s: no launch plan for M=%d N=%d with %d-column tiles", op, p.M, p.N, bn);
+    return HV_ERR_INVALID;
+  }
+  return cuda_status(launch_gemm(a0, a1, b, out, res, p, e, bn, plan, stream), op);
+}
+
 int op_gemm(const __half* A, int64_t lda, const __half* A2, int64_t lda2, int64_t K1, const __half* W, __half* out, int64_t ldc,
             int64_t M, int64_t N, int64_t K, const hv_epilogue* ep, cudaStream_t stream) {
-  const int sms = device_sms();
-  if (!sms) return HV_ERR_CUDA;
-  if (M <= 0 || N <= 0 || K <= 0 || (K % 8) || (lda % 8) || (ldc % 8) || (N % 8)) {
+  if (!A || !W || !out || M <= 0 || N <= 0 || K <= 0 || (K % 8) || (lda % 8) || (ldc % 8) || (N % 8)) {
     set_error("hv_op_gemm: bad shape M=%lld N=%lld K=%lld lda=%lld ldc=%lld", (long long)M, (long long)N, (long long)K, (long long)lda,
               (long long)ldc);
     return HV_ERR_INVALID;
@@ -159,6 +168,8 @@ int op_gemm(const __half* A, int64_t lda, const __half* A2, int64_t lda2, int64_
     return HV_ERR_INVALID;
   }
   if (int rc = check_epilogue_io("hv_op_gemm", out, ep)) return rc;
+  const int sms = device_sms();
+  if (!sms) return HV_ERR_CUDA;
   CUtensorMap ma0, ma1, mb;
   const int64_t Ka = split ? K1 : K;
   int bn;
@@ -172,20 +183,18 @@ int op_gemm(const __half* A, int64_t lda, const __half* A2, int64_t lda2, int64_
   fill_epilogue(e, ep, out, ldc, N);
   CUtensorMap mo, mr;
   if (int rc = make_epilogue_maps("hv_op_gemm", p, e, &mo, &mr)) return rc;
-  cudaError_t err = launch_gemm(ma0, ma1, mb, mo, mr, p, e, bn, sms, stream);
-  if (err != cudaSuccess) return cuda_fail(err, "hv_op_gemm launch");
-  return HV_OK;
+  return run_gemm("hv_op_gemm", ma0, ma1, mb, mo, mr, p, e, bn, sms, stream);
 }
 
 int op_gemm_batched_b(const __half* A, int64_t lda, const __half* X, int64_t ldx, __half* out, int64_t ldc, int64_t M, int64_t batch,
                       int64_t rows, int64_t out_stride, int64_t K, const __half* rowbias, cudaStream_t stream) {
-  const int sms = device_sms();
-  if (!sms) return HV_ERR_CUDA;
-  if (M <= 0 || batch <= 0 || rows <= 0 || (K % 8) || (lda % 8) || (ldx % 8) || (ldc % 8) || (out_stride % 8) || out_stride < rows) {
+  if (!A || !X || !out || M <= 0 || batch <= 0 || rows <= 0 || (K % 8) || (lda % 8) || (ldx % 8) || (ldc % 8) || (out_stride % 8) || out_stride < rows) {
     set_error("hv_op_gemm_batched_b: bad shape M=%lld batch=%lld rows=%lld stride=%lld K=%lld", (long long)M, (long long)batch, (long long)rows,
               (long long)out_stride, (long long)K);
     return HV_ERR_INVALID;
   }
+  const int sms = device_sms();
+  if (!sms) return HV_ERR_CUDA;
   CUtensorMap ma, mb;
   if (!make_map_2d(&ma, A, M, K, lda, 128)) { set_error("gemm_batched_b A map: %s", tma_last_error()); return HV_ERR_TMA; }
   const int64_t m_tiles = (M + 127) / 128;
@@ -204,9 +213,7 @@ int op_gemm_batched_b(const __half* A, int64_t lda, const __half* X, int64_t ldx
   e.ldc = static_cast<int>(ldc);
   e.n_valid = static_cast<int>(rows);
   e.rowbias = rowbias;
-  cudaError_t err = launch_gemm(ma, ma, mb, mb, mb, p, e, bn, sms, stream);
-  if (err != cudaSuccess) return cuda_fail(err, "hv_op_gemm_batched_b launch");
-  return HV_OK;
+  return run_gemm("hv_op_gemm_batched_b", ma, ma, mb, mb, mb, p, e, bn, sms, stream);
 }
 
 // Tiling of an implicit-GEMM convolution over the NF x H x W grid of the pixels it computes: one M tile is a box of frames x rows x columns.
@@ -223,14 +230,15 @@ static void set_conv_tiles(GemmProblem& p, int64_t NF, int64_t H, int64_t W) {
 
 int op_conv3x3(const __half* X, const __half* Wp, __half* out, int64_t ldc, int64_t NF, int64_t H, int64_t W, int64_t Cin,
                int64_t Cout, int stride, const hv_epilogue* ep, cudaStream_t stream, bool pad_end) {
-  const int sms = device_sms();
-  if (!sms) return HV_ERR_CUDA;
-  if ((Cin % 64) || (Cout % 8) || (ldc % 8) || (stride != 1 && stride != 2) || (pad_end && stride != 2) || NF <= 0 || H <= 0 || W <= 0) {
-    set_error("hv_op_conv3x3: bad shape NF=%lld H=%lld W=%lld Cin=%lld Cout=%lld stride=%d", (long long)NF, (long long)H, (long long)W,
-              (long long)Cin, (long long)Cout, stride);
+  if (!X || !Wp || !out || (Cin % 64) || (Cout % 8) || (ldc % 8) || (stride != 1 && stride != 2) || (pad_end && stride != 2) || NF <= 0 || H <= 0 ||
+      W <= 0) {
+    set_error("hv_op_conv3x3: bad shape NF=%lld H=%lld W=%lld Cin=%lld Cout=%lld stride=%d (or NULL pointer)", (long long)NF, (long long)H,
+              (long long)W, (long long)Cin, (long long)Cout, stride);
     return HV_ERR_INVALID;
   }
   if (int rc = check_epilogue_io("hv_op_conv3x3", out, ep)) return rc;
+  const int sms = device_sms();
+  if (!sms) return HV_ERR_CUDA;
   const int64_t Ho = stride == 1 ? H : H / 2, Wo = stride == 1 ? W : W / 2;
   GemmProblem p;
   p.a_mode = stride == 1 ? A_CONV3X3 : (pad_end ? A_CONV3X3_S2_END : A_CONV3X3_S2);
@@ -240,6 +248,10 @@ int op_conv3x3(const __half* X, const __half* Wp, __half* out, int64_t ldc, int6
   p.num_k_blocks = 9 * p.cin_blocks;
   set_conv_tiles(p, NF, Ho, Wo);
   const int bn = pick_block_n(Cout, (static_cast<int64_t>(NF) * Ho * Wo + 127) / 128, false, sms);
+  if (ep && ep->geglu && bn != 256) {   // the GEGLU epilogue pairs the [128 hidden | 128 gate] halves of a 256-column tile
+    set_error("hv_op_conv3x3: a geglu epilogue needs the 256-column tile, Cout=%lld gets %d columns", (long long)Cout, bn);
+    return HV_ERR_INVALID;
+  }
   CUtensorMap ma, mb;
   bool ok = stride == 1 ? make_map_nhwc(&ma, X, NF, H, W, Cin, p.bn, p.bh, p.bw) : make_map_nhwc_s2(&ma, X, NF, H, W, Cin, p.bn, p.bh, p.bw);
   if (!ok) { set_error("hv_op_conv3x3 X map: %s", tma_last_error()); return HV_ERR_TMA; }
@@ -248,22 +260,20 @@ int op_conv3x3(const __half* X, const __half* Wp, __half* out, int64_t ldc, int6
   fill_epilogue(e, ep, out, ldc, Cout);
   CUtensorMap mo, mr;
   if (int rc = make_epilogue_maps("hv_op_conv3x3", p, e, &mo, &mr)) return rc;
-  cudaError_t err = launch_gemm(ma, ma, mb, mo, mr, p, e, bn, sms, stream);
-  if (err != cudaSuccess) return cuda_fail(err, "hv_op_conv3x3 launch");
-  return HV_OK;
+  return run_gemm("hv_op_conv3x3", ma, ma, mb, mo, mr, p, e, bn, sms, stream);
 }
 
 // Nearest-2x upsample + 3x3 conv (Upsample3D, resnet.py:68-71 + :49) as four 2x2 convolutions of the SOURCE tensor, one per output
 // parity: the 4x larger upsampled tensor is never written or read and the conv does 4/9 of the multiply-adds.
 int op_upconv2x2(const __half* X, const __half* Wp, __half* out, int64_t ldc, int64_t NF, int64_t H, int64_t W, int64_t Cin, int64_t Cout,
                  const hv_epilogue* ep, cudaStream_t stream) {
-  const int sms = device_sms();
-  if (!sms) return HV_ERR_CUDA;
-  if ((Cin % 64) || (Cout % 8) || (ldc % 8) || NF <= 0 || H <= 0 || W <= 0 || (ep && (ep->residual || ep->rowvec || ep->geglu))) {
-    set_error("hv_op_upconv2x2: bad shape NF=%lld H=%lld W=%lld Cin=%lld Cout=%lld (or unsupported epilogue)", (long long)NF, (long long)H, (long long)W,
-              (long long)Cin, (long long)Cout);
+  if (!X || !Wp || !out || (Cin % 64) || (Cout % 8) || (ldc % 8) || NF <= 0 || H <= 0 || W <= 0 || (ep && (ep->residual || ep->rowvec || ep->geglu))) {
+    set_error("hv_op_upconv2x2: bad shape NF=%lld H=%lld W=%lld Cin=%lld Cout=%lld (or NULL pointer, unsupported epilogue)", (long long)NF, (long long)H,
+              (long long)W, (long long)Cin, (long long)Cout);
     return HV_ERR_INVALID;
   }
+  const int sms = device_sms();
+  if (!sms) return HV_ERR_CUDA;
   GemmProblem p;
   p.a_mode = A_UPCONV2X2;
   p.N = static_cast<int>(Cout);
@@ -280,9 +290,7 @@ int op_upconv2x2(const __half* X, const __half* Wp, __half* out, int64_t ldc, in
   if (!make_map_2d(&mb, Wp, 4 * Cout, 4 * Cin, 4 * Cin, bn)) { set_error("hv_op_upconv2x2 W map: %s", tma_last_error()); return HV_ERR_TMA; }
   GemmEpilogue e;
   fill_epilogue(e, ep, out, ldc, Cout);
-  cudaError_t err = launch_gemm(ma, ma, mb, mb, mb, p, e, bn, sms, stream);
-  if (err != cudaSuccess) return cuda_fail(err, "hv_op_upconv2x2 launch");
-  return HV_OK;
+  return run_gemm("hv_op_upconv2x2", ma, ma, mb, mb, mb, p, e, bn, sms, stream);
 }
 
 }  // namespace hv

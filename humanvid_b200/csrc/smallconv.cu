@@ -15,7 +15,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#include "kernels.h"
+#include "ops.h"
 #include "ptx.cuh"
 
 namespace hv {
@@ -245,47 +245,64 @@ __global__ void __launch_bounds__(256) pg_conv_in_kernel(const __half* __restric
 }
 
 template <int CIN, int COUT, int STRIDE>
-cudaError_t launch_sc(const __half* x, const __half* wp, const __half* bias, __half* out, int NF, int H, int W, int ldo, int act, cudaStream_t s) {
+int launch_sc(const __half* x, const __half* wp, const __half* bias, __half* out, int NF, int H, int W, int ldo, int act, cudaStream_t s) {
   using C = SCfg<CIN, COUT, STRIDE>;
   static bool attr = false;
   if (!attr) {
     cudaError_t e = cudaFuncSetAttribute(smallconv_mma_kernel<CIN, COUT, STRIDE>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmem);
-    if (e != cudaSuccess) return e;
+    if (e != cudaSuccess) return cuda_status(e, "hv_op_conv3x3_small");
     attr = true;
   }
   const int Ho = STRIDE == 1 ? H : H / 2, Wo = STRIDE == 1 ? W : W / 2;
   dim3 grid((Wo + SC_TW - 1) / SC_TW, (Ho + SC_TH - 1) / SC_TH, NF);
   smallconv_mma_kernel<CIN, COUT, STRIDE><<<grid, SC_THREADS, C::kSmem, s>>>(x, wp, bias, out, H, W, Ho, Wo, ldo, act);
-  return cudaGetLastError();
+  return cuda_status(cudaGetLastError(), "hv_op_conv3x3_small");
 }
 
 }  // namespace
 
-bool smallconv_supported(int cin, int cout, int stride) {
+bool smallconv_supported(int64_t cin, int64_t cout, int stride) {
   return (cin == 16 && cout == 16 && stride == 1) || (cin == 16 && cout == 32 && stride == 2) || (cin == 32 && cout == 32 && stride == 1) ||
          (cin == 32 && cout == 96 && stride == 2);
 }
 
-// x (NF, H, W, cin) channels-last, wp [cout][9 * cin] (launch_pack_conv3x3 with no padding), out (NF, Ho, Wo, ldo >= cout; pad columns untouched)
-cudaError_t launch_smallconv(const __half* x, const __half* wp, const __half* bias, __half* out, int NF, int H, int W, int cin, int cout, int stride,
-                             int ldo, int act, cudaStream_t s) {
-  if (stride == 2 && ((H | W) & 1)) return cudaErrorInvalidValue;
-  if (ldo % 8) return cudaErrorInvalidValue;
-  if (cin == 16 && cout == 16 && stride == 1) return launch_sc<16, 16, 1>(x, wp, bias, out, NF, H, W, ldo, act, s);
-  if (cin == 16 && cout == 32 && stride == 2) return launch_sc<16, 32, 2>(x, wp, bias, out, NF, H, W, ldo, act, s);
-  if (cin == 32 && cout == 32 && stride == 1) return launch_sc<32, 32, 1>(x, wp, bias, out, NF, H, W, ldo, act, s);
-  if (cin == 32 && cout == 96 && stride == 2) return launch_sc<32, 96, 2>(x, wp, bias, out, NF, H, W, ldo, act, s);
-  return cudaErrorInvalidValue;
+// x (NF, H, W, cin) channels-last, wp [cout][9 * cin] (op_pack_conv3x3 with no padding), out (NF, Ho, Wo, ldo >= cout; pad columns untouched).
+// x and wp are staged with 16-byte cp.async and out is written 16 bytes at a time; NF and the output's 8-row tiles are the grid's z and y.
+int op_conv3x3_small(const __half* x, const __half* wp, const __half* bias, __half* out, int64_t ldo, int64_t NF, int64_t H, int64_t W, int64_t cin,
+                     int64_t cout, int stride, int act, cudaStream_t s) {
+  if (!smallconv_supported(cin, cout, stride)) {
+    set_error("hv_op_conv3x3_small: (Cin, Cout, stride) = (%lld, %lld, %d) is not one of (16,16,1) (16,32,2) (32,32,1) (32,96,2)", (long long)cin,
+              (long long)cout, stride);
+    return HV_ERR_INVALID;
+  }
+  if (!x || !wp || !out || !aligned16(x) || !aligned16(wp) || !aligned16(out) || NF < 1 || NF > 65535 || H < 1 || W < 1 || H > INT32_MAX ||
+      W > INT32_MAX || (H / stride + SC_TH - 1) / SC_TH > 65535 || (stride == 2 && ((H | W) & 1)) || (ldo % 8) || ldo < cout || ldo > INT32_MAX) {
+    set_error("hv_op_conv3x3_small: bad arguments NF=%lld H=%lld W=%lld ldo=%lld (16-byte aligned X, Wp and out, 1 <= NF <= 65535, even H and W at "
+              "stride 2, ldo >= Cout and a multiple of 8)", (long long)NF, (long long)H, (long long)W, (long long)ldo);
+    return HV_ERR_INVALID;
+  }
+  const int n = static_cast<int>(NF), h = static_cast<int>(H), w = static_cast<int>(W), ld = static_cast<int>(ldo);
+  if (cin == 16 && cout == 16) return launch_sc<16, 16, 1>(x, wp, bias, out, n, h, w, ld, act, s);
+  if (cin == 16) return launch_sc<16, 32, 2>(x, wp, bias, out, n, h, w, ld, act, s);
+  if (cout == 32) return launch_sc<32, 32, 1>(x, wp, bias, out, n, h, w, ld, act, s);
+  return launch_sc<32, 96, 2>(x, wp, bias, out, n, h, w, ld, act, s);
 }
 
-cudaError_t launch_pg_conv_in(const __half* x, const __half* w, const __half* bias, __half* out, int B, int F, int H, int W, int act, int num_sms,
-                              cudaStream_t s) {
-  const int tiles_x = (W + PG_TW - 1) / PG_TW, tiles_y = (H + PG_TH - 1) / PG_TH;
-  long long blocks = static_cast<long long>(B) * F * tiles_y * tiles_x;
-  if (blocks > static_cast<long long>(num_sms) * 7) blocks = static_cast<long long>(num_sms) * 7;   // 7 x 28.6 KB of static shared memory per SM
-  if (blocks < 1) return cudaErrorInvalidValue;
-  pg_conv_in_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(x, w, bias, out, B, F, H, W, act, tiles_x, tiles_y);
-  return cudaGetLastError();
+// out (B*F, H, W, 16) is written 16 bytes at a time
+int op_pose_conv_in(const __half* x, const __half* w, const __half* bias, __half* out, int64_t B, int64_t F, int64_t H, int64_t W, int act, cudaStream_t s) {
+  if (!x || !w || !out || !aligned16(out) || B < 1 || F < 1 || H < 1 || W < 1 || B * F > INT32_MAX || H * W > INT32_MAX) {
+    set_error("hv_op_pose_conv_in: bad arguments B=%lld F=%lld H=%lld W=%lld (non-NULL X, W and out, 16-byte aligned out, B, F, H, W >= 1, B*F and "
+              "H*W within int32)", (long long)B, (long long)F, (long long)H, (long long)W);
+    return HV_ERR_INVALID;
+  }
+  const int sms = device_sms();
+  if (!sms) return HV_ERR_CUDA;
+  const int Hi = static_cast<int>(H), Wi = static_cast<int>(W);
+  const int tiles_x = (Wi + PG_TW - 1) / PG_TW, tiles_y = (Hi + PG_TH - 1) / PG_TH;
+  long long blocks = B * F * tiles_y * tiles_x;
+  if (blocks > static_cast<long long>(sms) * 7) blocks = static_cast<long long>(sms) * 7;   // 7 x 28.6 KB of static shared memory per SM
+  pg_conv_in_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(x, w, bias, out, static_cast<int>(B), static_cast<int>(F), Hi, Wi, act, tiles_x, tiles_y);
+  return cuda_status(cudaGetLastError(), "hv_op_pose_conv_in");
 }
 
 }  // namespace hv

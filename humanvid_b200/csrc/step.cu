@@ -13,9 +13,15 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#include "kernels.h"
+#include "ops.h"
 
 namespace hv {
+
+constexpr int kMaxWindows = 32;
+struct StepPreds {                       // window w's UNet prediction, (Bl, C, Fw, HW) fp16 each; cond unused without CFG
+  const __half* uncond[kMaxWindows];
+  const __half* cond[kMaxWindows];
+};
 
 namespace {
 
@@ -83,23 +89,49 @@ inline unsigned blocks_for(long long n, int num_sms) {
 
 }  // namespace
 
-cudaError_t launch_window_gather(const __half* latents, const int* idx, __half* out, int Bl, int C, int Ftot, int Fw, int HW, int R, int num_sms,
-                                 cudaStream_t s) {
-  const long long total = static_cast<long long>(Bl) * C * Fw * HW;
-  window_gather_kernel<<<blocks_for(total, num_sms), kThreads, 0, s>>>(latents, idx, out, Bl, C, Ftot, Fw, HW, R);
-  return cudaGetLastError();
+int op_window_gather(const __half* latents, const int32_t* idx, __half* out, int64_t Bl, int64_t C, int64_t Ftot, int64_t Fw, int64_t HW, int R,
+                     cudaStream_t s) {
+  if (!latents || !idx || !out || !int32_ok(Bl) || !int32_ok(C) || !int32_ok(Ftot) || !int32_ok(Fw) || !int32_ok(HW) || R < 1) {
+    set_error("hv_op_window_gather: bad argument (non-NULL pointers, Bl, C, Ftot, Fw, HW >= 1 within int32, repeat >= 1)");
+    return HV_ERR_INVALID;
+  }
+  const int sms = device_sms();
+  if (!sms) return HV_ERR_CUDA;
+  const long long total = Bl * C * Fw * HW;
+  window_gather_kernel<<<blocks_for(total, sms), kThreads, 0, s>>>(latents, idx, out, static_cast<int>(Bl), static_cast<int>(C), static_cast<int>(Ftot),
+                                                                    static_cast<int>(Fw), static_cast<int>(HW), R);
+  return cuda_status(cudaGetLastError(), "hv_op_window_gather");
 }
 
-cudaError_t launch_cfg_ddim_step(const StepPreds& preds, const int* inv, int K, const float* coef, const int* step_idx, __half* latents, int Bl, int C,
-                                 int Ftot, int Fw, int HW, float guidance, int cfg, int epsilon, int num_sms, cudaStream_t s) {
-  const long long total = static_cast<long long>(Bl) * C * Ftot * HW;
-  cfg_ddim_step_kernel<<<blocks_for(total, num_sms), kThreads, 0, s>>>(preds, inv, K, coef, step_idx, latents, Bl, C, Ftot, Fw, HW, guidance, cfg, epsilon);
-  return cudaGetLastError();
+// coef is read as float4
+int op_cfg_ddim_step(const void* const* pred_uncond, const void* const* pred_cond, int n_windows, const int32_t* inv, int K, const float* coef,
+                     const int32_t* step_index, __half* latents, int64_t Bl, int64_t C, int64_t Ftot, int64_t Fw, int64_t HW, float guidance_scale,
+                     int prediction_type, cudaStream_t s) {
+  if (!pred_uncond || !inv || !coef || !latents || n_windows < 1 || n_windows > kMaxWindows || K < 1 || (prediction_type != 0 && prediction_type != 1) ||
+      !aligned16(coef) || !int32_ok(Bl) || !int32_ok(C) || !int32_ok(Ftot) || !int32_ok(Fw) || !int32_ok(HW)) {
+    set_error("hv_op_cfg_ddim_step: bad argument (1..%d windows, prediction_type 0 = v_prediction / 1 = epsilon, 16-byte aligned coef, Bl, C, Ftot, "
+              "Fw, HW >= 1 within int32)", kMaxWindows);
+    return HV_ERR_INVALID;
+  }
+  StepPreds sp{};
+  for (int w = 0; w < n_windows; ++w) {
+    sp.uncond[w] = static_cast<const __half*>(pred_uncond[w]);
+    sp.cond[w] = pred_cond ? static_cast<const __half*>(pred_cond[w]) : nullptr;
+    if (!sp.uncond[w] || (pred_cond && !sp.cond[w])) { set_error("hv_op_cfg_ddim_step: window %d has a NULL prediction", w); return HV_ERR_INVALID; }
+  }
+  const int sms = device_sms();
+  if (!sms) return HV_ERR_CUDA;
+  const long long total = Bl * C * Ftot * HW;
+  cfg_ddim_step_kernel<<<blocks_for(total, sms), kThreads, 0, s>>>(sp, inv, K, coef, step_index, latents, static_cast<int>(Bl), static_cast<int>(C),
+                                                                    static_cast<int>(Ftot), static_cast<int>(Fw), static_cast<int>(HW), guidance_scale,
+                                                                    pred_cond ? 1 : 0, prediction_type);
+  return cuda_status(cudaGetLastError(), "hv_op_cfg_ddim_step");
 }
 
-cudaError_t launch_advance_index(int* idx, cudaStream_t s) {
+int op_advance_index(int32_t* idx, cudaStream_t s) {
+  if (!idx) { set_error("hv_op_advance_index: NULL index"); return HV_ERR_INVALID; }
   advance_index_kernel<<<1, 1, 0, s>>>(idx);
-  return cudaGetLastError();
+  return cuda_status(cudaGetLastError(), "hv_op_advance_index");
 }
 
 }  // namespace hv

@@ -46,7 +46,7 @@ enum hv_act { HV_ACT_NONE = 0, HV_ACT_RELU = 1, HV_ACT_SILU = 2, HV_ACT_QUICK_GE
 /* Fused epilogue of hv_op_gemm / hv_op_conv3x3, applied in this order in fp32 with ONE fp16 rounding at the store (the
  * reference's eager fp16 modules round after every step; the fp32 oracle is the parity anchor):  v = acc + bias;
  * v += rowvec[row / rows_per_group]; v = act(v); v += residual[row].  With geglu != 0 the packed weight holds [128 hidden | 128 gate] rows per 256-row block and the
- * output is hidden * gelu_erf(gate) with N/2 columns. */
+ * output is hidden * gelu_erf(gate) with N/2 columns (hv_op_conv3x3 runs geglu only where it picks the 256-column tile). */
 typedef struct hv_epilogue {
   const void* bias;      /* fp16 [N] or NULL */
   const void* rowvec;    /* fp16 [groups][rowvec_ld] or NULL (time-embedding projection per batch item) */
@@ -61,14 +61,16 @@ typedef struct hv_epilogue {
 
 /* out[M, N] = A[M, K] * W[N, K]^T (+epilogue).  A may be split column-wise over two buffers (torch.cat of a skip
  * connection is never materialised): columns [0,K1) come from A (row stride lda), [K1,K) from A2 (row stride lda2);
- * K1 = 0 / A2 = NULL means a single source.  K1 must be a multiple of 64. */
+ * K1 = 0 / A2 = NULL means a single source.  K1 must be a multiple of 64.  HV_ERR_INVALID for: A, W or out NULL, M, N or K <= 0, K, N, lda or ldc
+ * not a multiple of 8, a split with K1 % 64, lda2 % 8 or K1 >= K, geglu with N % 256, and the epilogue I/O hv_epilogue rejects. */
 int hv_op_gemm(const void* A, int64_t lda, const void* A2, int64_t lda2, int64_t K1, const void* W, void* out, int64_t ldc,
                int64_t M, int64_t N, int64_t K, const hv_epilogue* ep, hv_stream_t stream);
 
 /* out[M][n*out_stride + j] = sum_k A[M][k] * X[n][j][k], n < batch, j < rows: the "swapped" GEMM that yields V^T with every
  * frame's token segment starting on a 16-byte boundary (out_stride % 8 == 0), as TMA readers of V^T require.  The pad columns
  * [rows, round8(rows)) of each segment are written too, as 0 + rowbias[m] (0 without rowbias); columns [round8(rows), out_stride)
- * and [batch*out_stride, ldc) are left untouched. */
+ * and [batch*out_stride, ldc) are left untouched.  HV_ERR_INVALID for NULL A, X or out, M, batch or rows <= 0, K, lda, ldx, ldc or
+ * out_stride not a multiple of 8, and out_stride < rows. */
 int hv_op_gemm_batched_b(const void* A, int64_t lda, const void* X, int64_t ldx, void* out, int64_t ldc, int64_t M, int64_t batch,
                          int64_t rows, int64_t out_stride, int64_t K, const void* rowbias /* fp16 [M] added to row m, or NULL */,
                          hv_stream_t stream);
@@ -78,7 +80,10 @@ int hv_op_gemm_batched_b(const void* A, int64_t lda, const void* X, int64_t ldx,
  * {(16,16,1), (16,32,2), (32,32,1), (32,96,2)}, padding 1, + bias, act.  X (NF, H, W, Cin) channels-last; Wp = hv_pack_conv3x3 with
  * Cin_pad = Cin, Cout_pad = Cout ([Cout][9 * Cin]); out (NF, Ho, Wo, ldo >= Cout), columns >= Cout are left untouched.
  * hv_op_pose_conv_in: the PoseGuider's conv_in (3 -> 16) read straight from the (B, 3, F, H, W) image, W in the reference layout (16,3,3,3),
- * out channels-last (B*F, H, W, 16). */
+ * out channels-last (B*F, H, W, 16).
+ * HV_ERR_INVALID (hv_op_conv3x3_small) for: another (Cin, Cout, stride); X, Wp or out NULL or not 16-byte aligned; NF outside [1, 65535]; H or W
+ * < 1 or odd at stride 2; more than 65535 rows of 8 output rows; ldo < Cout or not a multiple of 8.
+ * HV_ERR_INVALID (hv_op_pose_conv_in) for: X, W or out NULL, out not 16-byte aligned, B, F, H or W < 1, B*F or H*W past int32. */
 int hv_op_conv3x3_small(const void* X, const void* Wp, const void* bias, void* out, int64_t ldo, int64_t NF, int64_t H, int64_t W, int64_t Cin,
                         int64_t Cout, int32_t stride, int32_t act, hv_stream_t stream);
 int hv_op_pose_conv_in(const void* X, const void* W, const void* bias, void* out, int64_t B, int64_t F, int64_t H, int64_t W_, int32_t act,
@@ -88,14 +93,17 @@ int hv_op_pose_conv_in(const void* X, const void* W, const void* bias, void* out
  * tensor: every output parity (2y+py, 2x+px) is a 2x2 convolution of the source whose weights are sums of the 3x3 taps that land on
  * the same source pixel (4/9 of the multiply-adds; the summed weights are rounded to fp16 once, at packing).
  * X (NF, H, W, Cin) -> out (NF, 2H, 2W, Cout) given as [rows][ldc]; Wp = hv_pack_upconv2x2(W (Cout, Cin, 3, 3)) : [4][Cout][4 * Cin].
- * Epilogue: bias only.  Cin % 64 == 0; Cout a multiple of the 128/160/256-column tile the GEMM picks (320, 640, 1280 are). */
+ * Epilogue: bias only.  Cin % 64 == 0; Cout a multiple of the 128/160/256-column tile the GEMM picks (320, 640, 1280 are).  HV_ERR_INVALID
+ * for NULL pointers, the shapes above and NF, H or W <= 0; hv_pack_upconv2x2 for NULL pointers and Cout or Cin outside [1, INT32_MAX]. */
 int hv_op_upconv2x2(const void* X, const void* Wp, void* out, int64_t ldc, int64_t NF, int64_t H, int64_t W, int64_t Cin, int64_t Cout,
                     const hv_epilogue* ep, hv_stream_t stream);
 int hv_pack_upconv2x2(const void* W, void* out, int64_t Cout, int64_t Cin, hv_stream_t stream);
 
 /* 3x3 convolution, padding 1, stride 1 or 2, over channels-last X (NF, H, W, Cin) -> out (NF, Ho, Wo, Cout) given as
  * a [rows][ldc] matrix.  Wp is the packed weight [Cout][9 * Cin] with k = (ky*3 + kx) * Cin + c (see hv_pack_conv3x3).
- * Cin must be a multiple of 64; stride 2 needs even H and W. */
+ * Cin must be a multiple of 64; stride 2 needs even H and W.  HV_ERR_INVALID for: X, Wp or out NULL, Cin % 64, Cout or ldc % 8, a stride
+ * other than 1 or 2, NF, H or W <= 0, the epilogue I/O hv_epilogue rejects, and a geglu epilogue when the GEMM picks a tile narrower than
+ * 256 columns for Cout. */
 int hv_op_conv3x3(const void* X, const void* Wp, void* out, int64_t ldc, int64_t NF, int64_t H, int64_t W, int64_t Cin,
                   int64_t Cout, int32_t stride, const hv_epilogue* ep, hv_stream_t stream);
 
@@ -112,14 +120,16 @@ int hv_op_conv3x3_s2_pad_end(const void* X, const void* Wp, void* out, int64_t l
 int hv_op_clip_patchify(const void* X, void* out, int64_t B, int64_t C, int64_t S, int64_t p, int64_t Kpad, hv_stream_t stream);
 
 /* Small-channel direct 3x3 convolution (any Cin/Cout, stride 1/2, padding 1) for conv_in and the PoseGuider stack.
- * W is the reference layout (Cout, Cin, 3, 3) fp16; act = hv_act. */
+ * W is the reference layout (Cout, Cin, 3, 3) fp16; act = hv_act.  HV_ERR_INVALID for: X, W or out NULL, a stride other than 1 or 2, NF < 1,
+ * H, W, Cin or Cout outside [1, INT32_MAX]. */
 int hv_op_conv3x3_direct(const void* X, const void* W, const void* bias, void* out, int64_t NF, int64_t H, int64_t Wd,
                          int64_t Cin, int64_t Cout, int32_t stride, int32_t act, const void* add, hv_stream_t stream);
 
 /* GroupNorm over (H*W, C/groups) per frame, fp32 statistics (summed relative to one input value of the group, so a large mean does not
  * cancel the variance); optional SiLU; reads the channel concatenation of X
  * (C1 channels) and X2 (C2 channels, may be NULL/0) and writes one (NF, HW, C1+C2) tensor. stats: fp32 scratch
- * of hv_groupnorm_scratch_floats(...) floats (per-slab partial sums; the reduction is atomics-free and deterministic). */
+ * of hv_groupnorm_scratch_floats(...) floats (per-slab partial sums; the reduction is atomics-free and deterministic).
+ * HV_ERR_INVALID, writing nothing, for what hv_op_groupnorm_pooled rejects at frames_per_item = 1. */
 size_t hv_groupnorm_scratch_floats(int64_t C, int64_t NF, int64_t HW, int32_t groups);
 int hv_op_groupnorm(const void* X, int64_t C1, const void* X2, int64_t C2, const void* gamma, const void* beta, void* out,
                     int64_t NF, int64_t HW, int32_t groups, float eps, int32_t silu, float* stats, hv_stream_t stream);
@@ -138,7 +148,8 @@ int hv_op_groupnorm_pooled(const void* X, int64_t C1, const void* X2, int64_t C2
 
 /* LayerNorm over C per row.  Optional: `pre_add` fp16 [rows / rows_per_group][C] is added to x first and the sum is
  * written to `x_out` (the cross-attention residual, see DESIGN.md); `pe` fp16 [F][C] is added to the normalised row
- * (row -> frame (row / hw) % F) as the motion module does before q/k/v. */
+ * (row -> frame (row / hw) % F) as the motion module does before q/k/v.  HV_ERR_INVALID for: X, gamma, beta or out NULL, any tensor
+ * (pre_add, x_out and pe included) not 16-byte aligned, rows < 1, C not a multiple of 8 in [8, 1280], hw or F past INT32_MAX. */
 int hv_op_layernorm(const void* X, const void* gamma, const void* beta, void* out, int64_t rows, int64_t C, float eps,
                     const void* pre_add, int64_t rows_per_group, void* x_out, const void* pe, int64_t hw, int64_t F,
                     hv_stream_t stream);
@@ -175,7 +186,8 @@ int hv_op_attention_d512(const void* Q, int64_t ldq, const void* K, int64_t ldk,
 int hv_op_temporal_attention(const void* QKV, void* out, int64_t B, int64_t F, int64_t HW, int32_t heads, int32_t d,
                              hv_stream_t stream);
 
-/* Layout / glue kernels. */
+/* Layout / glue kernels.  HV_ERR_INVALID for: NULL pointers, B, C, F, H or W < 1, H*W past int32, B*F > 65535 (ncfhw_to_nhwc,
+ * nhwc_to_ncfhw; also ldx < C), and for pixel_unshuffle r < 1 or not dividing H and W, or B*F, C*r*r past int32. */
 int hv_op_ncfhw_to_nhwc(const void* X, void* out, int64_t B, int64_t C, int64_t F, int64_t H, int64_t W, int32_t src_fp32,
                         hv_stream_t stream);
 int hv_op_nhwc_to_ncfhw(const void* X, int64_t ldx, void* out, int64_t B, int64_t C, int64_t F, int64_t H, int64_t W,
@@ -185,13 +197,16 @@ int hv_op_pixel_unshuffle(const void* X, void* out, int64_t B, int64_t C, int64_
 /* Plucker-embedding producer on the device (Camera + ray_condition, src/dataset/dance_image_h_v_camera.py:17-130; called from
  * scripts/pose2vid.py:52-84) fused with CameraPoseEncoder's PixelUnshuffle(r) (pose_adaptor.py:222,233-236):
  * K: DEVICE fp32 [NF][4] = (fx, fy, cx, cy) in pixels; c2w: DEVICE fp32 [NF][16] row-major camera-to-world (relative poses);
- * out: channels-last fp16 (NF, H/r, W/r, 6*r*r) with channel = c*r*r + dy*r + dx, i.e. pixel_unshuffle(plucker (NF, 6, H, W)). */
+ * out: channels-last fp16 (NF, H/r, W/r, 6*r*r) with channel = c*r*r + dy*r + dx, i.e. pixel_unshuffle(plucker (NF, 6, H, W)).
+ * HV_ERR_INVALID for NULL pointers, NF < 1, r < 1 or not dividing H and W, H or W past INT32_MAX. */
 int hv_op_plucker_unshuffle(const float* K, const float* c2w, void* out, int64_t NF, int64_t H, int64_t W, int32_t r, hv_stream_t stream);
 /* y[M][N] = act_in(x[M][K]) * W[N][K]^T + bias, tiny M (time embedding, cross-attention collapse); fp32 math,
- * fp16 rounding of the result. act_in: hv_act applied to x first. */
+ * fp16 rounding of the result. act_in: hv_act applied to x first.  HV_ERR_INVALID for: X, W or out NULL, X or W not 4-byte aligned, M, N,
+ * K outside [1, INT32_MAX], K odd, more than INT32_MAX blocks of 8 outputs. */
 int hv_op_small_linear(const void* X, const void* W, const void* bias, void* out, int64_t M, int64_t N, int64_t K,
                        int32_t act_in, hv_stream_t stream);
-/* Timesteps(320, flip_sin_to_cos=True, shift=0): out[b] = [cos(t w_i) | sin(t w_i)] rounded to fp16. */
+/* Timesteps(320, flip_sin_to_cos=True, shift=0): out[b] = [cos(t w_i) | sin(t w_i)] rounded to fp16.  HV_ERR_INVALID for NULL out, B < 1,
+ * dim < 2 or odd, B*dim past INT32_MAX. */
 int hv_op_timestep_embedding(int64_t timestep, void* out, int64_t B, int64_t dim, hv_stream_t stream);
 
 /* ---- per-timestep glue of Pose2VideoPipeline.__call__ on the device (src/pipelines/pipeline_pose2vid_long.py:516-563) ----
@@ -207,7 +222,9 @@ int hv_op_timestep_embedding(int64_t timestep, void* out, int64_t B, int64_t dim
  *   a window slot holding that frame, or -1; coef: DEVICE float [steps][4] = sqrt(a_t), sqrt(1-a_t), sqrt(a_prev),
  *   sqrt(1-a_prev); step_index: DEVICE int32 (row of coef used; NULL = row 0), read when the kernel runs so that a captured
  *   CUDA graph of one step replays for every timestep.
- * hv_op_advance_index: *index += 1 on the device (end of a graph-captured step). */
+ * hv_op_advance_index: *index += 1 on the device (end of a graph-captured step).
+ * HV_ERR_INVALID for NULL pointers (a NULL prediction of a window included), Bl, C, Ftot, Fw or HW outside [1, INT32_MAX], repeat < 1,
+ * n_windows outside [1, 32], K < 1, another prediction_type and a coef table not 16-byte aligned. */
 int hv_op_window_gather(const void* latents, const int32_t* frame_idx, void* out, int64_t Bl, int64_t C, int64_t Ftot, int64_t Fw, int64_t HW,
                         int32_t repeat, hv_stream_t stream);
 int hv_op_cfg_ddim_step(const void* const* pred_uncond, const void* const* pred_cond, int32_t n_windows, const int32_t* inv, int32_t K,
@@ -216,7 +233,8 @@ int hv_op_cfg_ddim_step(const void* const* pred_uncond, const void* const* pred_
 int hv_op_advance_index(int32_t* index, hv_stream_t stream);
 
 /* Weight packing (device to device).  conv: fp16 (Cout, Cin, 3, 3) -> [Cout_pad][9*Cin_pad] (zero padded); geglu: rows of a [8C][K] matrix
- * (and its bias) interleaved in 128-row hidden/gate blocks; heads: [heads*d][K] -> [heads*dpad][K] with zero rows. */
+ * (and its bias) interleaved in 128-row hidden/gate blocks; heads: [heads*d][K] -> [heads*dpad][K] with zero rows.  HV_ERR_INVALID for
+ * NULL pointers, sizes < 1 or past INT32_MAX, a padded size below its true size, and geglu rows not a multiple of 256. */
 int hv_pack_conv3x3(const void* W, void* out, int64_t Cout, int64_t Cin, int64_t Cout_pad, int64_t Cin_pad, hv_stream_t stream);
 int hv_pack_geglu(const void* W, void* out, int64_t rows, int64_t K, hv_stream_t stream);
 int hv_pack_heads(const void* W, void* out, int32_t heads, int32_t d, int32_t dpad, int64_t K, hv_stream_t stream);
