@@ -38,7 +38,7 @@ def build(force: bool = False, extra: list[str] | None = None, verbose: bool = F
         objs.append(obj)
         if not force and os.path.exists(obj) and os.path.getmtime(obj) > max(
             os.path.getmtime(os.path.join(CSRC, f)) for f in os.listdir(CSRC) if f.endswith((".h", ".cuh")) or os.path.join(CSRC, f) == src
-        ) and os.path.getmtime(obj) > os.path.getmtime(os.path.join(HERE, "..", "include", "hv_b200_ops.h")):
+        ) and os.path.getmtime(obj) > max(os.path.getmtime(os.path.join(HERE, "..", "include", f)) for f in ("hv_b200_ops.h", "hv_b200_fp8.h")):
             continue
         cmd = [NVCC, *FLAGS, *(extra or []), "-x", "cu", "-c", src, "-o", obj]
         procs.append((src, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))

@@ -1,4 +1,5 @@
 // extern "C" operator entry points declared in include/hv_b200_ops.h: each is the checked operator function of ops.h.
+#include "../../include/hv_b200_fp8.h"
 #include "../../include/hv_b200_ops.h"
 #include "ops.h"
 
@@ -126,6 +127,20 @@ int hv_op_cfg_ddim_step(const void* const* pred_uncond, const void* const* pred_
 }
 int hv_op_advance_index(int32_t* index, hv_stream_t stream) {
   return op_advance_index(index, ST(stream));
+}
+
+int hv_op_gemm_fp8(const void* A, int64_t lda, const float* a_scale, int64_t a_scale_ld, const void* W, const float* w_scale, void* out,
+                   int64_t ldc, float* out_scale, int64_t out_scale_ld, int64_t M, int64_t N, int64_t K, const hv_epilogue* ep, hv_stream_t stream) {
+  return op_gemm_fp8(static_cast<const uint8_t*>(A), lda, a_scale, a_scale_ld, static_cast<const uint8_t*>(W), w_scale, out, ldc, out_scale,
+                     out_scale_ld, M, N, K, ep, ST(stream));
+}
+int hv_op_layernorm_fp8(const void* X, const void* gamma, const void* beta, void* out, float* out_scale, int64_t rows, int64_t C, float eps,
+                        const void* pre_add, int64_t rows_per_group, void* x_out, const void* pe, int64_t hw, int64_t F, hv_stream_t stream) {
+  return op_layernorm_fp8(H(X), H(gamma), H(beta), static_cast<uint8_t*>(out), out_scale, rows, C, eps, H(pre_add), rows_per_group, HM(x_out), H(pe),
+                          hw, F, ST(stream));
+}
+int hv_pack_fp8_rows(const void* W, void* out, float* scale, int64_t rows, int64_t K, hv_stream_t stream) {
+  return op_pack_fp8_rows(H(W), static_cast<uint8_t*>(out), scale, rows, K, ST(stream));
 }
 
 int hv_dbg_gemm(const void* A, int64_t lda, const void* W, float* out, int64_t M, int64_t N, int64_t K, hv_stream_t stream) {

@@ -96,12 +96,14 @@ __device__ __forceinline__ float2 ldh2(const __half* p) { return __half22float2(
 // BST ("B-stationary"): every tile a CTA visits has the same n_blk (the host makes gridDim.x a multiple of n_tiles), so
 // the CTA loads its BLOCK_N x K weight panel into shared memory once and streams only A afterwards.  For the K <= 640
 // linears of the two high-resolution levels this removes the per-tile re-fetch of B from L2.
-template <int BLOCK_N, bool BST>
+// FP8: e4m3 operands (A_LINEAR only).  A k-block is then 128 values: the same 128-byte swizzled rows, ring and descriptors.
+template <int BLOCK_N, bool BST, bool FP8>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ CUtensorMap map_a1,
             const __grid_constant__ CUtensorMap map_b, const __grid_constant__ CUtensorMap map_out,
             const __grid_constant__ CUtensorMap map_res, const GemmProblem p, const GemmEpilogue e) {
   using C = Cfg<BLOCK_N>;
+  constexpr int KB = FP8 ? 2 * BLOCK_K : BLOCK_K;   // elements per k-block
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int nstages = p.stages;
@@ -152,7 +154,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ 
       if (BST && static_cast<int>(blockIdx.x) < num_tiles) {
         mbar_arrive_expect_tx(bar_bpanel, nkb * C::kBTileBytes);
         for (int kb = 0; kb < nkb; ++kb)
-          tma_load_2d(smem + kb * C::kBTileBytes, &map_b, bar_bpanel, kb * BLOCK_K, (blockIdx.x % n_tiles) * BLOCK_N);
+          tma_load_2d(smem + kb * C::kBTileBytes, &map_b, bar_bpanel, kb * KB, (blockIdx.x % n_tiles) * BLOCK_N);
       }
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int m_blk = tile / n_tiles, n_blk = tile % n_tiles;
@@ -164,9 +166,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ 
           mbar_arrive_expect_tx(&bar_full[stage], kRingStageBytes);
           if (p.a_mode == A_LINEAR) {
             if (p.k_split == 0 || kb < p.k_split)
-              tma_load_2d(sa, &map_a0, &bar_full[stage], kb * BLOCK_K, tc.m0);
+              tma_load_2d(sa, &map_a0, &bar_full[stage], kb * KB, tc.m0);
             else
-              tma_load_2d(sa, &map_a1, &bar_full[stage], (kb - p.k_split) * BLOCK_K, tc.m0);
+              tma_load_2d(sa, &map_a1, &bar_full[stage], (kb - p.k_split) * KB, tc.m0);
           } else {
             const int tap = kb / p.cin_blocks, cb = kb - tap * p.cin_blocks;
             const int dy = tap / 3, dx = tap - dy * 3;
@@ -188,9 +190,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ 
           }
           if (!BST) {
             if (p.b_batch)
-              tma_load_3d(sb, &map_b, &bar_full[stage], kb * BLOCK_K, (n_blk % n_per_batch) * BLOCK_N, n_blk / n_per_batch);
+              tma_load_3d(sb, &map_b, &bar_full[stage], kb * KB, (n_blk % n_per_batch) * BLOCK_N, n_blk / n_per_batch);
             else
-              tma_load_2d(sb, &map_b, &bar_full[stage], kb * BLOCK_K, n_blk * BLOCK_N + (tc.py * 2 + tc.px) * p.b_par_rows);
+              tma_load_2d(sb, &map_b, &bar_full[stage], kb * KB, n_blk * BLOCK_N + (tc.py * 2 + tc.px) * p.b_par_rows);
           }
           if (++stage == nstages) { stage = 0; phase ^= 1; }
         }
@@ -251,12 +253,57 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ 
     float acc[BLOCK_N / 2];
 #pragma unroll
     for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
+    // FP8 with per-(row, k-block) A scales: the k-block's products go to `part` and are promoted into acc scaled by
+    // s_a[row, kb] once its MMAs are complete (this also keeps the FP8 MMA's own limited-precision accumulation to one k-block).
+    // Two accumulator sets fit beside the epilogue at BLOCK_N <= 160 only; the host never asks for it at 256.
+    // launch_gemm_fp8 refuses per-block A scales at BLOCK_N = 256, where this kernel would compute without them.
+    constexpr bool kPromote = FP8 && BLOCK_N <= 160;
+    [[maybe_unused]] float part[kPromote ? BLOCK_N / 2 : 1];
+    [[maybe_unused]] const float* sa_row[2] = {nullptr, nullptr};
+    if constexpr (kPromote) {
+      if (e.a_scale_ld) {
+#pragma unroll
+        for (int i = 0; i < BLOCK_N / 2; ++i) part[i] = 0.f;
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const int row = m_blk * BLOCK_M + wg * 64 + wq * 16 + (lane >> 2) + 8 * hh;
+          sa_row[hh] = row < p.M ? e.a_scale + static_cast<long long>(row) * e.a_scale_ld : nullptr;
+        }
+      }
+    }
     int prev_stage = -1;
     for (int kb = 0; kb < nkb; ++kb) {
       mbar_wait(&bar_full[stage], phase);
       const uint32_t sa = smem_u32(ring + stage * kRingStageBytes);
       const uint64_t adesc = gmma_desc_k_sw128(sa + wg * (A_TILE_BYTES / 2));
       const uint64_t bdesc = gmma_desc_k_sw128(BST ? smem_u32(smem + kb * C::kBTileBytes) : sa + A_TILE_BYTES);
+      if constexpr (FP8) {
+        bool promoted = false;
+        if constexpr (kPromote) {
+          if (e.a_scale_ld) {
+            wgmma_fence_regs(part);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < KB / 32; ++k) wgmma_ss_e4m3<BLOCK_N>(part, adesc + 2 * k, bdesc + 2 * k, k ? 1u : 0u);
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_regs(part);
+            const float s0 = sa_row[0] ? __ldg(sa_row[0] + kb) : 0.f, s1 = sa_row[1] ? __ldg(sa_row[1] + kb) : 0.f;
+#pragma unroll
+            for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = fmaf((i & 2) ? s1 : s0, part[i], acc[i]);
+            promoted = true;
+          }
+        }
+        if (!promoted) {
+          wgmma_fence_regs(acc);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < KB / 32; ++k) wgmma_ss_e4m3<BLOCK_N>(acc, adesc + 2 * k, bdesc + 2 * k, 1u);
+          wgmma_commit();
+          wgmma_wait<1>();
+          wgmma_fence_regs(acc);
+        }
+      } else {
       wgmma_fence_regs(acc);
       wgmma_fence();
 #pragma unroll
@@ -264,6 +311,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ 
       wgmma_commit();
       wgmma_wait<1>();                     // the previous k-block's MMAs are complete: its ring slot may be refilled
       wgmma_fence_regs(acc);
+      }
       if (prev_stage >= 0 && lane == 0) mbar_arrive(&bar_empty[prev_stage]);
       prev_stage = stage;
       if (++stage == nstages) { stage = 0; phase ^= 1; }
@@ -283,6 +331,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ 
       bool ok[2];
       const __half* rv[2];
       int rt[2];
+      [[maybe_unused]] float rs[2];   // FP8: the per-row A scale (1 when the k-blocks were promoted with theirs)
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
         rt[hh] = wg * 64 + wq * 16 + (lane >> 2) + 8 * hh;
@@ -298,6 +347,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ 
           row = (static_cast<long long>(n) * p.H + y) * p.W + x;
         }
         rv[hh] = e.rowvec != nullptr && ok[hh] ? e.rowvec + (row / e.rows_per_group) * e.rowvec_ld : nullptr;
+        if constexpr (FP8) rs[hh] = e.a_scale_ld == 0 && ok[hh] ? __ldg(e.a_scale + row) : 1.f;
       }
       const bool res = e.residual != nullptr;
       const float rowbias = 0.f;
@@ -328,6 +378,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ 
               if (col < e.n_valid) {
                 uint32_t* w = reinterpret_cast<uint32_t*>(slab + rt[hh] * 64 + ((jj ^ ((rt[hh] >> 1) & 3)) << 4) + 4 * quad);
                 float v0 = acc[4 * j + 2 * hh] + rowbias, v1 = acc[4 * j + 2 * hh + 1] + rowbias;
+                if constexpr (FP8) {
+                  const float2 sw = __ldg(reinterpret_cast<const float2*>(e.w_scale + col));
+                  v0 = acc[4 * j + 2 * hh] * rs[hh] * sw.x;
+                  v1 = acc[4 * j + 2 * hh + 1] * rs[hh] * sw.y;
+                }
                 if (has_bias) {
                   const float2 b = ldh2(e.bias + col);
                   v0 += b.x;
@@ -379,6 +434,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ 
       const __half* __restrict__ res = e.residual != nullptr ? e.residual + row * e.ldr : nullptr;
       const float rowbias = e.rowbias != nullptr ? __half2float(e.rowbias[row]) : 0.f;
       __half* __restrict__ out = e.out + row * e.ldc;
+      [[maybe_unused]] float rs = 1.f;
+      if constexpr (FP8) rs = e.a_scale_ld == 0 ? __ldg(e.a_scale + row) : 1.f;
       if (!e.geglu) {
         const int tile_col0 = p.b_batch ? (n_blk / n_per_batch) * p.b_out_stride + (n_blk % n_per_batch) * BLOCK_N : n_blk * BLOCK_N;
         const int col_lim = p.b_batch ? (n_blk / n_per_batch) * p.b_out_stride + ((p.b_rows + 7) & ~7) : e.n_valid;
@@ -387,6 +444,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ 
           const int col = tile_col0 + 8 * j + 2 * quad;
           if (col < col_lim) {
             float v0 = acc[4 * j + 2 * hh] + rowbias, v1 = acc[4 * j + 2 * hh + 1] + rowbias;
+            if constexpr (FP8) {
+              const float2 sw = __ldg(reinterpret_cast<const float2*>(e.w_scale + col));
+              v0 = acc[4 * j + 2 * hh] * rs * sw.x;
+              v1 = acc[4 * j + 2 * hh + 1] * rs * sw.y;
+            }
             if (has_bias) {
               const float2 b = ldh2(e.bias + col);
               v0 += b.x;
@@ -414,6 +476,45 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ 
             }
             *reinterpret_cast<uint32_t*>(out + col) = pack_h2(v0, v1);
           }
+        }
+      } else if constexpr (FP8) {
+        // GEGLU on dequantised accumulators; with out8 the 128 outputs of the row are quantised to e4m3 with one scale, their amax
+        // reduced over the quad of lanes that hold the row (the geglu value replaces the hidden accumulator it came from)
+        float amax = 0.f;
+#pragma unroll
+        for (int j = 0; j < BLOCK_N / 16; ++j) {
+          const int hcol = n_blk * BLOCK_N + 8 * j + 2 * quad;
+          const int ocol = n_blk * (BLOCK_N / 2) + 8 * j + 2 * quad;
+          const float2 swh = __ldg(reinterpret_cast<const float2*>(e.w_scale + hcol));
+          const float2 swg = __ldg(reinterpret_cast<const float2*>(e.w_scale + hcol + BLOCK_N / 2));
+          float h0 = acc[4 * j + 2 * hh] * rs * swh.x, h1 = acc[4 * j + 2 * hh + 1] * rs * swh.y;
+          float g0 = acc[4 * (j + BLOCK_N / 16) + 2 * hh] * rs * swg.x, g1 = acc[4 * (j + BLOCK_N / 16) + 2 * hh + 1] * rs * swg.y;
+          if (has_bias) {
+            const float2 bh = ldh2(e.bias + hcol), bg = ldh2(e.bias + hcol + BLOCK_N / 2);
+            h0 += bh.x;
+            h1 += bh.y;
+            g0 += bg.x;
+            g1 += bg.y;
+          }
+          const float o0 = geglu1(h0, g0), o1 = geglu1(h1, g1);
+          if (e.out8 != nullptr) {
+            acc[4 * j + 2 * hh] = o0;
+            acc[4 * j + 2 * hh + 1] = o1;
+            amax = fmaxf(amax, fmaxf(fabsf(o0), fabsf(o1)));
+          } else if (ocol < e.n_valid) {
+            *reinterpret_cast<uint32_t*>(out + ocol) = pack_h2(o0, o1);
+          }
+        }
+        if (e.out8 != nullptr) {
+          const unsigned qmask = 0xFu << (lane & 28);
+          amax = fmaxf(amax, __shfl_xor_sync(qmask, amax, 1));
+          amax = fmaxf(amax, __shfl_xor_sync(qmask, amax, 2));
+          const float inv = e4m3_inv(amax);
+          uint8_t* o8 = e.out8 + row * e.ldc + n_blk * (BLOCK_N / 2);
+#pragma unroll
+          for (int j = 0; j < BLOCK_N / 16; ++j)
+            *reinterpret_cast<uint16_t*>(o8 + 8 * j + 2 * quad) = e4m3x2(acc[4 * j + 2 * hh], acc[4 * j + 2 * hh + 1], inv);
+          if (quad == 0) e.out8_scale[row * e.out8_scale_ld + n_blk] = e4m3_scale(amax);
         }
       } else {
         // GEGLU (BLOCK_N == 256): tile columns [0,128) are "hidden", [128,256) the matching "gate" rows of the packed weight
@@ -492,20 +593,20 @@ static int smem_bytes(int block_n, bool bst, int num_k_blocks, int stages, int s
   return (bst ? num_k_blocks * btile : 0) + stages * (A_TILE_BYTES + (bst ? 0 : btile)) + slabs * SLAB_BYTES + (2 * kMaxStages + 3) * 8 + 1024;
 }
 
-template <int BN, bool BST>
+template <int BN, bool BST, bool FP8>
 static cudaError_t launch_t(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const CUtensorMap& out, const CUtensorMap& res,
                             GemmProblem p, const GemmEpilogue& e, const GemmPlan& plan, cudaStream_t stream) {
   static_assert(Cfg<BN>::kFixed == (2 * kMaxStages + 3) * 8 + 1024, "plan_smem and the kernel lay out the barriers alike");
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t err = cudaFuncSetAttribute(gemm_kernel<BN, BST>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
+    cudaError_t err = cudaFuncSetAttribute(gemm_kernel<BN, BST, FP8>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
     if (err != cudaSuccess) return err;
     attr_set = true;
   }
   p.stages = plan.stages;
   p.epi_slabs = plan.epi_slabs;
   const int smem = smem_bytes(BN, BST, p.num_k_blocks, plan.stages, plan.epi_slabs);
-  gemm_kernel<BN, BST><<<plan.grid, GEMM_THREADS, smem, stream>>>(a0, a1, b, out, res, p, e);
+  gemm_kernel<BN, BST, FP8><<<plan.grid, GEMM_THREADS, smem, stream>>>(a0, a1, b, out, res, p, e);
   return cudaGetLastError();
 }
 
@@ -540,13 +641,27 @@ bool plan_gemm(const GemmProblem& p, int block_n, int num_sms, GemmPlan* plan) {
 cudaError_t launch_gemm(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const CUtensorMap& out, const CUtensorMap& res,
                         const GemmProblem& p, const GemmEpilogue& e, int block_n, const GemmPlan& plan, cudaStream_t stream) {
   if (plan.bst_stages > 0) {
-    if (block_n == 256) return launch_t<256, true>(a0, a1, b, out, res, p, e, plan, stream);
-    if (block_n == 160) return launch_t<160, true>(a0, a1, b, out, res, p, e, plan, stream);
-    return launch_t<128, true>(a0, a1, b, out, res, p, e, plan, stream);
+    if (block_n == 256) return launch_t<256, true, false>(a0, a1, b, out, res, p, e, plan, stream);
+    if (block_n == 160) return launch_t<160, true, false>(a0, a1, b, out, res, p, e, plan, stream);
+    return launch_t<128, true, false>(a0, a1, b, out, res, p, e, plan, stream);
   }
-  if (block_n == 256) return launch_t<256, false>(a0, a1, b, out, res, p, e, plan, stream);
-  if (block_n == 160) return launch_t<160, false>(a0, a1, b, out, res, p, e, plan, stream);
-  return launch_t<128, false>(a0, a1, b, out, res, p, e, plan, stream);
+  if (block_n == 256) return launch_t<256, false, false>(a0, a1, b, out, res, p, e, plan, stream);
+  if (block_n == 160) return launch_t<160, false, false>(a0, a1, b, out, res, p, e, plan, stream);
+  return launch_t<128, false, false>(a0, a1, b, out, res, p, e, plan, stream);
+}
+
+cudaError_t launch_gemm_fp8(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& out, const CUtensorMap& res, const GemmProblem& p,
+                            const GemmEpilogue& e, int block_n, const GemmPlan& plan, cudaStream_t stream) {
+  // the 256-wide instantiations have no second accumulator set: they would ignore per-(row, k-block) A scales
+  if (e.a_scale_ld != 0 && block_n == 256) return cudaErrorInvalidValue;
+  if (plan.bst_stages > 0) {
+    if (block_n == 256) return launch_t<256, true, true>(a, a, b, out, res, p, e, plan, stream);
+    if (block_n == 160) return launch_t<160, true, true>(a, a, b, out, res, p, e, plan, stream);
+    return launch_t<128, true, true>(a, a, b, out, res, p, e, plan, stream);
+  }
+  if (block_n == 256) return launch_t<256, false, true>(a, a, b, out, res, p, e, plan, stream);
+  if (block_n == 160) return launch_t<160, false, true>(a, a, b, out, res, p, e, plan, stream);
+  return launch_t<128, false, true>(a, a, b, out, res, p, e, plan, stream);
 }
 
 }  // namespace hv

@@ -25,6 +25,13 @@ struct GemmEpilogue {
   int act = ACT_NONE;
   int geglu = 0;                   // BLOCK_N=256 tile = [128 hidden | 128 gate] -> 128 outputs
   const __half* rowbias = nullptr; // [M]: added to every column of output row m (the "ones" rows of V^T)
+  // e4m3 GEMMs only (launch_gemm_fp8): acc is dequantised first, D = w_scale[n] * (a_scale * acc), then the steps above
+  const float* a_scale = nullptr;  // a_scale_ld == 0: [M], one per row; else [M][a_scale_ld], one per (row, 128-k block)
+  int a_scale_ld = 0;
+  const float* w_scale = nullptr;  // [N] (packed order)
+  uint8_t* out8 = nullptr;         // GEGLU only: e4m3 output [rows][ldc] instead of out, one scale per 128 output columns in
+  float* out8_scale = nullptr;     //   out8_scale[row * out8_scale_ld + column / 128]
+  int out8_scale_ld = 0;
 };
 
 struct GemmProblem {
@@ -66,6 +73,12 @@ bool plan_gemm(const GemmProblem& p, int block_n, int num_sms, GemmPlan* plan);
 // block_n must be 128, 160 or 256 (256 required for geglu); 160 = two exact tiles for the 320-wide layers.  plan: plan_gemm(p, block_n).
 cudaError_t launch_gemm(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const CUtensorMap& out, const CUtensorMap& res,
                         const GemmProblem& p, const GemmEpilogue& e, int block_n, const GemmPlan& plan, cudaStream_t stream);
+// The same kernel on e4m3 operands (A_LINEAR only): a k-block is 128 e4m3 values (p.num_k_blocks = ceil(K / 128)), the maps are
+// make_map_2d_e4m3 maps, and e.a_scale / e.w_scale dequantise the fp32 accumulators.  Per-(row, 128-k block) A scales
+// (e.a_scale_ld > 0) need block_n 128 or 160: each k-block's products land in a second accumulator set and are added into the main
+// one scaled by a_scale.
+cudaError_t launch_gemm_fp8(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& out, const CUtensorMap& res, const GemmProblem& p,
+                            const GemmEpilogue& e, int block_n, const GemmPlan& plan, cudaStream_t stream);
 
 // Picks the (bn, bh, bw) output-tile box of 128 output pixels with the least padding for an NF x H x W output
 // (every box dimension is a power of two <= 128).

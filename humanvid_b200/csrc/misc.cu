@@ -279,6 +279,40 @@ __global__ void clip_patchify_kernel(const __half* __restrict__ x, __half* __res
   }
 }
 
+// e4m3 rows with one scale each (the FP8 weights: s_w[n] = amax(row n) / 448): one warp per row, 8 values per lane and step; the
+// second pass re-reads the row from L2.
+__global__ void pack_fp8_rows_kernel(const __half* __restrict__ w, uint8_t* __restrict__ out, float* __restrict__ scale, int rows, int K) {
+  const int lane = threadIdx.x & 31;
+  const long long row = static_cast<long long>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= rows) return;
+  const __half* src = w + row * K;
+  float amax = 0.f;
+  for (int c = lane * 8; c < K; c += 256) {
+    const uint4 u = __ldg(reinterpret_cast<const uint4*>(src + c));
+    const __half2* h = reinterpret_cast<const __half2*>(&u);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float2 f = __half22float2(h[j]);
+      amax = fmaxf(amax, fmaxf(fabsf(f.x), fabsf(f.y)));
+    }
+  }
+#pragma unroll
+  for (int o = 16; o; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+  const float inv = e4m3_inv(amax);
+  for (int c = lane * 8; c < K; c += 256) {
+    const uint4 u = __ldg(reinterpret_cast<const uint4*>(src + c));
+    const __half2* h = reinterpret_cast<const __half2*>(&u);
+    uint32_t q[2];
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const float2 f0 = __half22float2(h[2 * j]), f1 = __half22float2(h[2 * j + 1]);
+      q[j] = e4m3x2(f0.x, f0.y, inv) | (static_cast<uint32_t>(e4m3x2(f1.x, f1.y, inv)) << 16);
+    }
+    *reinterpret_cast<uint2*>(out + row * K + c) = make_uint2(q[0], q[1]);
+  }
+  if (lane == 0) scale[row] = e4m3_scale(amax);
+}
+
 }  // namespace
 
 // Each operator below rejects NULL pointers and sizes its kernel would narrow out of int32 (or, where a size becomes gridDim.y / .z,
@@ -415,6 +449,13 @@ int op_pack_heads(const __half* w, __half* out, int heads, int d, int dpad, int6
   const long long total = static_cast<long long>(heads) * dpad * K;
   pack_heads_kernel<<<blocks_for(total, sms), kThreads, 0, s>>>(w, out, total, d, dpad, static_cast<int>(K));
   return cuda_status(cudaGetLastError(), "hv_pack_heads");
+}
+int op_pack_fp8_rows(const __half* w, uint8_t* out, float* scale, int64_t rows, int64_t K, cudaStream_t s) {
+  if (!w || !out || !scale || !aligned16(w) || !aligned16(out) || !aligned16(scale) || !int32_ok(rows) || !int32_ok(K) || (K % 16))
+    return invalid("hv_pack_fp8_rows", "non-NULL, 16-byte aligned pointers, rows >= 1 and K a positive multiple of 16 within int32");
+  constexpr int kWarps = 8;
+  pack_fp8_rows_kernel<<<static_cast<unsigned>((rows + kWarps - 1) / kWarps), kWarps * 32, 0, s>>>(w, out, scale, static_cast<int>(rows), static_cast<int>(K));
+  return cuda_status(cudaGetLastError(), "hv_pack_fp8_rows");
 }
 int op_dbg_gemm(const __half* a, int64_t lda, const __half* w, float* out, int64_t M, int64_t N, int64_t K, cudaStream_t s) {
   if (!a || !w || !out || !int32_ok(M) || !int32_ok(N) || !int32_ok(K) || M * N > INT32_MAX)

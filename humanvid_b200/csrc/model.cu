@@ -14,6 +14,7 @@
 #include <memory>
 #include <string>
 #include <unordered_map>
+#include <tuple>
 #include <vector>
 
 #include "../../include/hv_b200.h"
@@ -67,6 +68,8 @@ struct Lin {
   Mat w;
   __half* bias = nullptr;
   bool geglu = false;  // packed by ff1_geglu: runs with the GEGLU epilogue, w.rows / 2 outputs
+  uint8_t* w8 = nullptr;  // FP8 mode: e4m3 copy of w (hv_pack_fp8_rows), one scale per packed row in sw; the linear then runs on e4m3
+  float* sw = nullptr;
 };
 struct Conv3 {       // implicit-GEMM packed 3x3 conv
   Mat w;             // [cout_pad][9 * cin_pad]
@@ -84,6 +87,12 @@ struct Tens {  // channels-last activation
   int NF = 0, H = 0, W = 0, C = 0;
   int64_t rows() const { return static_cast<int64_t>(NF) * H * W; }
   int64_t numel() const { return rows() * C; }
+};
+struct Q8 {   // e4m3 activation of Tens t's shape (t.p unused): one scale per row (sld == 0) or per (row, 128 columns), s[row * sld + j]
+  Tens t;
+  uint8_t* q = nullptr;
+  float* s = nullptr;
+  int sld = 0;
 };
 
 struct ResnetW {
@@ -390,6 +399,15 @@ struct hv_model {
     l.geglu = true;
     return l;
   }
+  // FP8 mode (hv_config.fp8_linears): the transformer feed-forwards LN -> FF1 -> FF2 of width C >= 1280 run on e4m3.  They are the only
+  // covered shapes measured faster than fp16 (DESIGN.md §9); every other linear stays fp16.  The camera encoder and the other networks
+  // have no FP8 mode.
+  bool fp8_ff(int C) const { return cfg.kind == HV_KIND_UNET3D && cfg.fp8_linears && C >= 1280; }
+  void add_fp8(Lin& l) {
+    l.w8 = reinterpret_cast<uint8_t*>(dmalloc((l.w.rows * l.w.cols + 1) / 2));
+    l.sw = reinterpret_cast<float*>(dmalloc(2 * l.w.rows));
+    ckop(op_pack_fp8_rows(l.w.p, l.w8, l.sw, l.w.rows, l.w.cols, st), "pack fp8 rows");
+  }
 
   // temb == 0: a resnet without time embedding (no time_emb_proj)
   ResnetW resnet(const std::string& pfx, int cin, int cout, int temb, float eps = 1e-5f) {
@@ -460,6 +478,7 @@ struct hv_model {
     s.out2 = lin(b + ".attn2.to_out.0", C, C);
     s.ff1 = ff1_geglu(b + ".ff.net.0.proj", C);
     s.ff2 = lin(b + ".ff.net.2", C, 4 * C);
+    if (fp8_ff(C)) { add_fp8(s.ff1); add_fp8(s.ff2); }
     return s;
   }
   TAttnW tattn(const std::string& attn_pfx, const std::string& norm_pfx, int C) {
@@ -483,6 +502,7 @@ struct hv_model {
     b.ff_norm = norm(pfx + ".ff_norm", C, 1e-5f);
     b.ff1 = ff1_geglu(pfx + ".ff.net.0.proj", C);
     b.ff2 = lin(pfx + ".ff.net.2", C, 4 * C);
+    if (fp8_ff(C)) { add_fp8(b.ff1); add_fp8(b.ff2); }
     return b;
   }
   MotionW motion(const std::string& pfx, int C) {
@@ -732,6 +752,54 @@ struct hv_model {
     return out;
   }
 
+  // out = e4m3(LN(x (+ pre_add per batch item)) (+ pe per frame)), one scale per row
+  Q8 op_ln8(const Tens& x, const Norm& n, const __half* pre_add = nullptr, int64_t rows_per_b = 1, const __half* pe = nullptr, int F = 1) {
+    Q8 out;
+    out.t = x;
+    out.t.p = nullptr;
+    out.q = static_cast<uint8_t*>(ar.alloc(static_cast<size_t>(x.numel())));
+    out.s = static_cast<float*>(ar.alloc(sizeof(float) * x.rows()));
+    launch(1, {CAT_NORM, "layernorm_fp8", 0, x.rows(), x.C, 0}, [&] {
+      ckop(op_layernorm_fp8(x.p, n.g, n.b, out.q, out.s, x.rows(), x.C, n.eps, pre_add, rows_per_b, nullptr, pe, x.H * x.W, F, st), "layernorm fp8");
+    });
+    return out;
+  }
+  // e4m3 linear of an e4m3 activation: fp16 out (+ bias, + rowvec[row / rows_per_group], + res), or, for a GEGLU-packed weight, e4m3 out
+  // with one scale per 128 columns (the A operand of the next e4m3 linear)
+  Tens op_linear8(const Q8& x, const Lin& l, const Tens* res = nullptr, const __half* rowvec = nullptr, int64_t rows_per_group = 1) {
+    if (l.geglu) fail(HV_ERR_INVALID, "e4m3 linear with fp16 output: the weight is GEGLU-packed");
+    return std::get<0>(run_linear8(x, l, res, rowvec, rows_per_group));
+  }
+  Q8 op_geglu8(const Q8& x, const Lin& l) {
+    if (!l.geglu) fail(HV_ERR_INVALID, "e4m3 GEGLU: the weight is not GEGLU-packed");
+    return std::get<1>(run_linear8(x, l, nullptr, nullptr, 1));
+  }
+  std::tuple<Tens, Q8> run_linear8(const Q8& x, const Lin& l, const Tens* res, const __half* rowvec, int64_t rows_per_group) {
+    if (!l.w8) fail(HV_ERR_INVALID, "e4m3 linear: the weight has no e4m3 copy");
+    if (l.w.cols != x.t.C) fail(HV_ERR_INVALID, "e4m3 linear: input width %d != weight cols %lld", x.t.C, (long long)l.w.cols);
+    const int N = static_cast<int>(l.geglu ? l.w.rows / 2 : l.w.rows);
+    Tens out;
+    Q8 out8;
+    if (l.geglu) {
+      out8.t = x.t;
+      out8.t.C = N;
+      out8.t.p = nullptr;
+      out8.sld = N / 128;
+      out8.q = static_cast<uint8_t*>(ar.alloc(static_cast<size_t>(out8.t.numel())));
+      out8.s = static_cast<float*>(ar.alloc(sizeof(float) * out8.t.rows() * out8.sld));
+    } else {
+      out = alloc_act(x.t.NF, x.t.H, x.t.W, N);
+    }
+    hv_epilogue ep = epilogue(l.bias, res, HV_ACT_NONE, rowvec, rows_per_group, N);
+    ep.geglu = l.geglu ? 1 : 0;
+    launch(1, {CAT_GEMM, l.geglu ? "gemm_geglu_fp8" : "gemm_fp8", 2.0 * x.t.rows() * l.w.rows * l.w.cols, x.t.rows(), l.w.rows, l.w.cols}, [&] {
+      ckop(op_gemm_fp8(x.q, x.t.C, x.s, x.sld, l.w8, l.sw, l.geglu ? static_cast<void*>(out8.q) : static_cast<void*>(out.p), l.geglu ? N : out.C,
+                       l.geglu ? out8.s : nullptr, out8.sld, x.t.rows(), l.w.rows, l.w.cols, &ep, st),
+           "gemm fp8");
+    });
+    return {out, out8};
+  }
+
   // The GEMM / conv wrappers write into `dst` (a tensor of the output's shape allocated by the caller) or into a new tensor.  Their
   // epilogue: + bias, + rowvec[row / rows_per_group] (rows of the output's width), act, + res.
   Tens dest(const Tens* dst, int NF, int H, int W, int C) {
@@ -904,10 +972,8 @@ struct hv_model {
     __half* ca = op_small_linear(v2, w.out2, B, HV_ACT_NONE);
     // LayerNorm-3 normalises t2 = t1 + ca[b] without writing t2: the same per-batch vector is added again, in fp32, in FF2's epilogue
     // (t3 = ff2(.) + bias + ca[b] + t1), which saves one full-tensor write per block and one rounding of the residual stream
-    Tens n3 = op_ln(t1, w.ln3, ca, static_cast<int64_t>(F) * L);
     // ---- feed-forward, proj_out + residual
-    Tens ffh = op_linear(n3, w.ff1);
-    Tens t3 = op_linear(ffh, w.ff2, &t1, nullptr, HV_ACT_NONE, nullptr, ca, static_cast<int64_t>(F) * L);
+    Tens t3 = ff_fwd(t1, w.ln3, w.ff1, w.ff2, ca, static_cast<int64_t>(F) * L);
     return op_linear(t3, w.proj_out, &x, &out);
   }
 
@@ -927,9 +993,14 @@ struct hv_model {
   // TemporalTransformerBlock: the temporal attentions, then t = ff(LN(t)) + t
   Tens tblock_fwd(const TBlockW& b, Tens t, int B, int F) {
     for (const auto& a : b.attn) t = tattn_fwd(a, t, B, F, b.heads, b.d);
-    Tens n = op_ln(t, b.ff_norm);
-    Tens ffh = op_linear(n, b.ff1);
-    return op_linear(ffh, b.ff2, &t);
+    return ff_fwd(t, b.ff_norm, b.ff1, b.ff2);
+  }
+  // x + ff2(GEGLU ff1(LN(x + pre_add[b]))) + pre_add[b] (pre_add per batch item of rows_per_b rows, or none): on e4m3 when the weights carry
+  // an e4m3 copy (fp8_ff), with the LayerNorm and GEGLU writing e4m3 and their scales
+  Tens ff_fwd(const Tens& x, const Norm& n, const Lin& ff1, const Lin& ff2, const __half* pre_add = nullptr, int64_t rows_per_b = 1) {
+    if (ff1.w8) return op_linear8(op_geglu8(op_ln8(x, n, pre_add, rows_per_b), ff1), ff2, &x, pre_add, rows_per_b);
+    Tens ffh = op_linear(op_ln(x, n, pre_add, rows_per_b), ff1);
+    return op_linear(ffh, ff2, &x, nullptr, HV_ACT_NONE, nullptr, pre_add, rows_per_b);
   }
 
   // VanillaTemporalModule (motion_module.py:44-259)

@@ -296,10 +296,13 @@ __global__ void gn_apply_pooled_kernel(const __half* __restrict__ x1, int C1, co
 // ---------------------------------------------------------------- LayerNorm: one warp per row
 // LPR lanes cooperate on one row (32/LPR rows per warp), each lane owning up to 5 vectors of 8 halves: C = 320 -> 8 lanes
 // x 5 vectors, 640 -> 16 x 5, 1280 -> 32 x 5, so every lane is busy and five 16-byte loads per lane are in flight.
-template <int LPR>
+// FP8: the normalised fp32 row (after affine and pe) is quantised to e4m3 into out8 [rows][C] with one scale per row, out_scale[row]
+// (ptx.cuh e4m3_inv / e4m3_scale); out is not written.
+template <int LPR, bool FP8>
 __global__ void __launch_bounds__(256) layernorm_kernel(const __half* __restrict__ x, const __half* __restrict__ gamma, const __half* __restrict__ beta,
                                  __half* __restrict__ out, long long rows, int C, float eps, const __half* __restrict__ pre_add,
-                                 long long rows_per_group, __half* __restrict__ x_out, const __half* __restrict__ pe, int hw, int F) {
+                                 long long rows_per_group, __half* __restrict__ x_out, const __half* __restrict__ pe, int hw, int F,
+                                 uint8_t* __restrict__ out8, float* __restrict__ out_scale) {
   constexpr int MAXV = 5;
   constexpr int RPW = 32 / LPR;   // rows per warp
   const int lane = threadIdx.x & 31;
@@ -372,8 +375,30 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const __half* __restrict
 #pragma unroll
         for (int j = 0; j < 8; ++j) v[k][j] += pv[j];
       }
-      *reinterpret_cast<uint4*>(out + row * C + vi * 8) = pack8(v[k]);
+      if constexpr (!FP8) *reinterpret_cast<uint4*>(out + row * C + vi * 8) = pack8(v[k]);
     }
+  }
+  if constexpr (FP8) {
+    float amax = 0.f;
+#pragma unroll
+    for (int k = 0; k < MAXV; ++k)
+      if (row_ok && sub + LPR * k < vecs)
+#pragma unroll
+        for (int j = 0; j < 8; ++j) amax = fmaxf(amax, fabsf(v[k][j]));
+#pragma unroll
+    for (int o = LPR / 2; o; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+    const float inv = e4m3_inv(amax);
+#pragma unroll
+    for (int k = 0; k < MAXV; ++k) {
+      const int vi = sub + LPR * k;
+      if (row_ok && vi < vecs) {
+        uint2 q;
+        q.x = e4m3x2(v[k][0], v[k][1], inv) | (static_cast<uint32_t>(e4m3x2(v[k][2], v[k][3], inv)) << 16);
+        q.y = e4m3x2(v[k][4], v[k][5], inv) | (static_cast<uint32_t>(e4m3x2(v[k][6], v[k][7], inv)) << 16);
+        *reinterpret_cast<uint2*>(out8 + row * C + vi * 8) = q;
+      }
+    }
+    if (row_ok && sub == 0) out_scale[row] = e4m3_scale(amax);
   }
   }
 }
@@ -539,14 +564,10 @@ int op_groupnorm_pooled(const __half* x1, int64_t C1, const __half* x2, int64_t 
 }
 
 // The kernel holds up to 160 vectors of 8 per row (C <= 1280) and loads x, pre_add, gamma, beta and pe and stores out and x_out 16 bytes at a time.
-int op_layernorm(const __half* x, const __half* gamma, const __half* beta, __half* out, int64_t rows, int64_t C, float eps, const __half* pre_add,
-                 int64_t rows_per_group, __half* x_out, const __half* pe, int64_t hw, int64_t F, cudaStream_t stream) {
-  if (!x || !gamma || !beta || !out || !aligned16(x) || !aligned16(gamma) || !aligned16(beta) || !aligned16(out) || !aligned16(pre_add) ||
-      !aligned16(x_out) || !aligned16(pe) || rows < 1 || C < 8 || C > 1280 || C % 8 || hw > INT32_MAX || F > INT32_MAX) {
-    set_error("hv_op_layernorm: bad arguments rows=%lld C=%lld hw=%lld F=%lld (non-NULL, 16-byte aligned tensors, rows >= 1, C a multiple of 8 "
-              "<= 1280, hw and F <= INT32_MAX)", (long long)rows, (long long)C, (long long)hw, (long long)F);
-    return HV_ERR_INVALID;
-  }
+template <bool FP8>
+static int run_layernorm(const char* op, const __half* x, const __half* gamma, const __half* beta, __half* out, int64_t rows, int64_t C, float eps,
+                         const __half* pre_add, int64_t rows_per_group, __half* x_out, const __half* pe, int64_t hw, int64_t F, uint8_t* out8,
+                         float* out_scale, cudaStream_t stream) {
   const int vecs = static_cast<int>(C / 8);
   if (rows_per_group <= 0) rows_per_group = 1;
   if (hw <= 0) hw = 1;
@@ -561,12 +582,36 @@ int op_layernorm(const __half* x, const __half* gamma, const __half* beta, __hal
   const unsigned grid = static_cast<unsigned>(blocks);
   const int Ci = static_cast<int>(C), hwi = static_cast<int>(hw), Fi = static_cast<int>(F);
   if (lpr == 8)
-    layernorm_kernel<8><<<grid, wpb * 32, 0, stream>>>(x, gamma, beta, out, rows, Ci, eps, pre_add, rows_per_group, x_out, pe, hwi, Fi);
+    layernorm_kernel<8, FP8><<<grid, wpb * 32, 0, stream>>>(x, gamma, beta, out, rows, Ci, eps, pre_add, rows_per_group, x_out, pe, hwi, Fi, out8, out_scale);
   else if (lpr == 16)
-    layernorm_kernel<16><<<grid, wpb * 32, 0, stream>>>(x, gamma, beta, out, rows, Ci, eps, pre_add, rows_per_group, x_out, pe, hwi, Fi);
+    layernorm_kernel<16, FP8><<<grid, wpb * 32, 0, stream>>>(x, gamma, beta, out, rows, Ci, eps, pre_add, rows_per_group, x_out, pe, hwi, Fi, out8, out_scale);
   else
-    layernorm_kernel<32><<<grid, wpb * 32, 0, stream>>>(x, gamma, beta, out, rows, Ci, eps, pre_add, rows_per_group, x_out, pe, hwi, Fi);
-  return cuda_status(cudaGetLastError(), "hv_op_layernorm");
+    layernorm_kernel<32, FP8><<<grid, wpb * 32, 0, stream>>>(x, gamma, beta, out, rows, Ci, eps, pre_add, rows_per_group, x_out, pe, hwi, Fi, out8, out_scale);
+  return cuda_status(cudaGetLastError(), op);
+}
+
+int op_layernorm(const __half* x, const __half* gamma, const __half* beta, __half* out, int64_t rows, int64_t C, float eps, const __half* pre_add,
+                 int64_t rows_per_group, __half* x_out, const __half* pe, int64_t hw, int64_t F, cudaStream_t stream) {
+  if (!x || !gamma || !beta || !out || !aligned16(x) || !aligned16(gamma) || !aligned16(beta) || !aligned16(out) || !aligned16(pre_add) ||
+      !aligned16(x_out) || !aligned16(pe) || rows < 1 || C < 8 || C > 1280 || C % 8 || hw > INT32_MAX || F > INT32_MAX) {
+    set_error("hv_op_layernorm: bad arguments rows=%lld C=%lld hw=%lld F=%lld (non-NULL, 16-byte aligned tensors, rows >= 1, C a multiple of 8 "
+              "<= 1280, hw and F <= INT32_MAX)", (long long)rows, (long long)C, (long long)hw, (long long)F);
+    return HV_ERR_INVALID;
+  }
+  return run_layernorm<false>("hv_op_layernorm", x, gamma, beta, out, rows, C, eps, pre_add, rows_per_group, x_out, pe, hw, F, nullptr, nullptr, stream);
+}
+
+int op_layernorm_fp8(const __half* x, const __half* gamma, const __half* beta, uint8_t* out, float* out_scale, int64_t rows, int64_t C, float eps,
+                     const __half* pre_add, int64_t rows_per_group, __half* x_out, const __half* pe, int64_t hw, int64_t F, cudaStream_t stream) {
+  if (!x || !gamma || !beta || !out || !out_scale || !aligned16(x) || !aligned16(gamma) || !aligned16(beta) || !aligned16(out) ||
+      !aligned16(out_scale) || !aligned16(pre_add) || !aligned16(x_out) || !aligned16(pe) || rows < 1 || C < 16 || C > 1280 || C % 16 ||
+      hw > INT32_MAX || F > INT32_MAX) {
+    set_error("hv_op_layernorm_fp8: bad arguments rows=%lld C=%lld hw=%lld F=%lld (non-NULL out and out_scale, 16-byte aligned tensors, rows >= 1, "
+              "C a multiple of 16 <= 1280, hw and F <= INT32_MAX)", (long long)rows, (long long)C, (long long)hw, (long long)F);
+    return HV_ERR_INVALID;
+  }
+  return run_layernorm<true>("hv_op_layernorm_fp8", x, gamma, beta, nullptr, rows, C, eps, pre_add, rows_per_group, x_out, pe, hw, F, out, out_scale,
+                             stream);
 }
 
 }  // namespace hv

@@ -186,6 +186,78 @@ int op_gemm(const __half* A, int64_t lda, const __half* A2, int64_t lda2, int64_
   return run_gemm("hv_op_gemm", ma0, ma1, mb, mo, mr, p, e, bn, sms, stream);
 }
 
+// e4m3 linear: the checks, then the kernel of op_gemm with KB = 128.  Tile width: GEGLU takes 256 (unpromoted, DESIGN §9); per-128 A
+// scales need a second accumulator set, so 160 or 128, whichever pads N less (ties to 160: N = 320, 640 -> 160, 1280 -> 160); per-row
+// scales follow pick_block_n as fp16 does.
+int op_gemm_fp8(const uint8_t* A, int64_t lda, const float* a_scale, int64_t a_scale_ld, const uint8_t* W, const float* w_scale, void* out,
+                int64_t ldc, float* out_scale, int64_t out_scale_ld, int64_t M, int64_t N, int64_t K, const hv_epilogue* ep, cudaStream_t stream) {
+  const char* op = "hv_op_gemm_fp8";
+  if (!A || !a_scale || !W || !w_scale || !out || !int32_ok(M) || !int32_ok(N) || !int32_ok(K) || (K % 16) || (N % 8) || lda < K || (lda % 16) ||
+      !aligned16(A) || !aligned16(W) || !aligned16(a_scale) || !aligned16(w_scale) || !aligned16(out_scale)) {
+    set_error("%s: bad arguments M=%lld N=%lld K=%lld lda=%lld (non-NULL A, a_scale, W, w_scale and out; 16-byte aligned pointers; K and lda >= K "
+              "multiples of 16, N of 8)", op, (long long)M, (long long)N, (long long)K, (long long)lda);
+    return HV_ERR_INVALID;
+  }
+  const int64_t kblocks = (K + 127) / 128;
+  if (a_scale_ld != 0 && (a_scale_ld < kblocks || a_scale_ld > INT32_MAX)) {
+    set_error("%s: a_scale_ld=%lld must be 0 (one scale per row) or >= ceil(K / 128) = %lld", op, (long long)a_scale_ld, (long long)kblocks);
+    return HV_ERR_INVALID;
+  }
+  const bool geglu = ep && ep->geglu;
+  if (geglu && ((N % 256) || a_scale_ld != 0)) {
+    set_error("%s: geglu needs N %% 256 == 0 (N=%lld) and one A scale per row", op, (long long)N);
+    return HV_ERR_INVALID;
+  }
+  if (out_scale) {
+    if (!geglu || ep->residual || ep->rowvec || ep->act || ep->n_valid || (ldc % 16) || ldc < N / 2 || out_scale_ld < N / 256 ||
+        out_scale_ld > INT32_MAX || !aligned16(out)) {
+      set_error("%s: an e4m3 output (out_scale != NULL) needs a geglu epilogue without residual, rowvec, act or n_valid, a 16-byte aligned out, "
+                "ldc >= N/2 a multiple of 16 and out_scale_ld >= N/256 (ldc=%lld out_scale_ld=%lld)", op, (long long)ldc, (long long)out_scale_ld);
+      return HV_ERR_INVALID;
+    }
+  } else {
+    if (ldc % 8) {
+      set_error("%s: ldc=%lld must be a multiple of 8", op, (long long)ldc);
+      return HV_ERR_INVALID;
+    }
+    if (int rc = check_epilogue_io(op, out, ep)) return rc;
+  }
+  const int sms = device_sms();
+  if (!sms) return HV_ERR_CUDA;
+  GemmProblem p;
+  p.M = static_cast<int>(M);
+  p.N = static_cast<int>(N);
+  p.num_k_blocks = static_cast<int>(kblocks);
+  p.a_mode = A_LINEAR;
+  const int bn = a_scale_ld ? ((N + 159) / 160 * 160 <= (N + 127) / 128 * 128 ? 160 : 128) : pick_block_n(N, (M + 127) / 128, geglu, sms);
+  CUtensorMap ma, mb;
+  if (!make_map_2d_e4m3(&ma, A, M, K, lda, 128)) { set_error("%s A map: %s", op, tma_last_error()); return HV_ERR_TMA; }
+  if (!make_map_2d_e4m3(&mb, W, N, K, K, bn)) { set_error("%s W map: %s", op, tma_last_error()); return HV_ERR_TMA; }
+  GemmEpilogue e;
+  e.a_scale = a_scale;
+  e.a_scale_ld = static_cast<int>(a_scale_ld);
+  e.w_scale = w_scale;
+  CUtensorMap mo = mb, mr = mb;
+  if (out_scale) {
+    e.ldc = static_cast<int>(ldc);
+    e.n_valid = static_cast<int>(N / 2);
+    e.bias = static_cast<const __half*>(ep->bias);
+    e.geglu = 1;
+    e.out8 = static_cast<uint8_t*>(out);
+    e.out8_scale = out_scale;
+    e.out8_scale_ld = static_cast<int>(out_scale_ld);
+  } else {
+    fill_epilogue(e, ep, static_cast<__half*>(out), ldc, N);
+    if (int rc = make_epilogue_maps(op, p, e, &mo, &mr)) return rc;
+  }
+  GemmPlan plan;
+  if (!plan_gemm(p, bn, sms, &plan) || (out_scale && plan.epi_slabs)) {
+    set_error("%s: no launch plan for M=%d N=%d with %d-column tiles", op, p.M, p.N, bn);
+    return HV_ERR_INVALID;
+  }
+  return cuda_status(launch_gemm_fp8(ma, mb, mo, mr, p, e, bn, plan, stream), op);
+}
+
 int op_gemm_batched_b(const __half* A, int64_t lda, const __half* X, int64_t ldx, __half* out, int64_t ldc, int64_t M, int64_t batch,
                       int64_t rows, int64_t out_stride, int64_t K, const __half* rowbias, cudaStream_t stream) {
   if (!A || !X || !out || M <= 0 || batch <= 0 || rows <= 0 || (K % 8) || (lda % 8) || (ldx % 8) || (ldc % 8) || (out_stride % 8) || out_stride < rows) {

@@ -6,6 +6,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "../../include/hv_b200_fp8.h"
 #include "../../include/hv_b200_ops.h"
 
 namespace hv {
@@ -24,6 +25,9 @@ int plan_linear(int64_t M, int64_t N, int64_t K, bool geglu, int* block_n, int* 
 int op_gemm(const __half* A, int64_t lda, const __half* A2, int64_t lda2, int64_t K1, const __half* W, __half* out, int64_t ldc,
             int64_t M, int64_t N, int64_t K, const hv_epilogue* ep, cudaStream_t stream);
 // out[M][n*out_stride + j] = sum_k A[M][k] * X[n][j][k] for n < batch, j < rows (X: [batch][rows][ldx]); out_stride % 8 == 0.
+// e4m3 operands with fp32 scales (hv_op_gemm_fp8): out is fp16 [M][ldc], or e4m3 [M][ldc] with out_scale for a GEGLU epilogue.
+int op_gemm_fp8(const uint8_t* A, int64_t lda, const float* a_scale, int64_t a_scale_ld, const uint8_t* W, const float* w_scale, void* out,
+                int64_t ldc, float* out_scale, int64_t out_scale_ld, int64_t M, int64_t N, int64_t K, const hv_epilogue* ep, cudaStream_t stream);
 int op_gemm_batched_b(const __half* A, int64_t lda, const __half* X, int64_t ldx, __half* out, int64_t ldc, int64_t M, int64_t batch,
                       int64_t rows, int64_t out_stride, int64_t K, const __half* rowbias, cudaStream_t stream);
 // pad_end (stride 2 only): padding (0, 1, 0, 1) instead of 1 on every side -- F.pad(x, (0, 1, 0, 1)) then a stride-2 conv with padding 0.
@@ -58,6 +62,8 @@ int op_groupnorm_pooled(const __half* X, int64_t C1, const __half* X2, int64_t C
                         int64_t NF, int64_t HW, int groups, float eps, int silu, int64_t F, float* stats, cudaStream_t stream);
 int op_layernorm(const __half* X, const __half* gamma, const __half* beta, __half* out, int64_t rows, int64_t C, float eps, const __half* pre_add,
                  int64_t rows_per_group, __half* x_out, const __half* pe, int64_t hw, int64_t F, cudaStream_t stream);
+int op_layernorm_fp8(const __half* X, const __half* gamma, const __half* beta, uint8_t* out, float* out_scale, int64_t rows, int64_t C, float eps,
+                     const __half* pre_add, int64_t rows_per_group, __half* x_out, const __half* pe, int64_t hw, int64_t F, cudaStream_t stream);
 // CLIP vision embeddings: row (b, t) of B x L tokens = LayerNorm((t == 0 ? cls : patch[b * (L - 1) + t - 1]) + pos[t]); rows = B * L.
 int op_clip_embed_ln(const __half* patch, const __half* cls, const __half* pos, const __half* gamma, const __half* beta, __half* out, int64_t rows,
                      int64_t L, int64_t C, float eps, cudaStream_t stream);
@@ -81,6 +87,7 @@ int op_pack_conv3x3(const __half* W, __half* out, int64_t Cout, int64_t Cin, int
 int op_pack_upconv2x2(const __half* W, __half* out, int64_t Cout, int64_t Cin, cudaStream_t stream);
 int op_pack_geglu(const __half* W, __half* out, int64_t rows, int64_t K, cudaStream_t stream);
 int op_pack_heads(const __half* W, __half* out, int heads, int d, int dpad, int64_t K, cudaStream_t stream);
+int op_pack_fp8_rows(const __half* W, uint8_t* out, float* scale, int64_t rows, int64_t K, cudaStream_t stream);
 int op_dbg_gemm(const __half* A, int64_t lda, const __half* W, float* out, int64_t M, int64_t N, int64_t K, cudaStream_t stream);
 
 // ---- small-channel convolutions of the PoseGuider front (smallconv.cu)

@@ -136,4 +136,17 @@ __device__ __forceinline__ float geglu1(float h, float g) {
   return h * (fmaxf(g, 0.f) - q);
 }
 
+// ---------------------------------------------------------------- e4m3 quantisation (the FP8 linears, DESIGN §9)
+// One step for every e4m3 producer, each an IEEE fp32 operation so that a CPU emulation reproduces the bytes from the same fp32
+// values: inv = 448 / amax, q = e4m3(x * inv) rounded to nearest even and saturated to +-448, s = amax / 448.  amax == 0 gives
+// inv = 0 (zero bytes) and s = 0.
+__device__ __forceinline__ float e4m3_inv(float amax) { return amax > 0.f ? __fdiv_rn(448.f, amax) : 0.f; }
+__device__ __forceinline__ float e4m3_scale(float amax) { return __fdiv_rn(amax, 448.f); }
+// e4m3(a * inv) in the low byte, e4m3(b * inv) in the high byte
+__device__ __forceinline__ uint16_t e4m3x2(float a, float b, float inv) {
+  uint16_t r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(__fmul_rn(b, inv)), "f"(__fmul_rn(a, inv)));
+  return r;
+}
+
 }  // namespace hv

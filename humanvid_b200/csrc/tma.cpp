@@ -20,14 +20,15 @@ void resolve() {
 }
 
 bool encode(CUtensorMap* m, const void* ptr, int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
-            const cuuint32_t* box, CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B) {
+            const cuuint32_t* box, CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B,
+            CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_FLOAT16) {
   std::call_once(g_once, resolve);
   if (!g_encode) {
     snprintf(g_err, sizeof g_err, "cuTensorMapEncodeTiled entry point not available");
     return false;
   }
   cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-  CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, rank, const_cast<void*>(ptr), dims, strides_bytes, box, estr,
+  CUresult r = g_encode(m, dtype, rank, const_cast<void*>(ptr), dims, strides_bytes, box, estr,
                         CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
@@ -51,6 +52,13 @@ bool make_map_2d_box(CUtensorMap* m, const void* ptr, int64_t rows, int64_t cols
 
 bool make_map_2d(CUtensorMap* m, const void* ptr, int64_t rows, int64_t cols, int64_t ld, int box_rows) {
   return make_map_2d_box(m, ptr, rows, cols, ld, box_rows, 64);
+}
+
+bool make_map_2d_e4m3(CUtensorMap* m, const void* ptr, int64_t rows, int64_t cols, int64_t ld, int box_rows) {
+  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  cuuint64_t strides[1] = {(cuuint64_t)ld};
+  cuuint32_t box[2] = {128, (cuuint32_t)box_rows};
+  return encode(m, ptr, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_DATA_TYPE_UINT8);
 }
 
 bool make_map_3d(CUtensorMap* m, const void* ptr, int64_t batch, int64_t rows, int64_t cols, int64_t ld, int box_rows) {

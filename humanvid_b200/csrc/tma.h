@@ -14,6 +14,10 @@ bool make_map_2d(CUtensorMap* m, const void* ptr, int64_t rows, int64_t cols, in
 // Same with an explicit box width (<= 64 columns).
 bool make_map_2d_box(CUtensorMap* m, const void* ptr, int64_t rows, int64_t cols, int64_t ld, int box_rows, int box_cols);
 
+// e4m3 row-major matrix [rows][ld] (ld in bytes, a multiple of 16) of which `cols` columns are valid; box = box_rows x 128 columns
+// (128-byte rows, the same 128B-swizzled tile as the fp16 box of 64 columns).  Out-of-bounds box elements read as zero.
+bool make_map_2d_e4m3(CUtensorMap* m, const void* ptr, int64_t rows, int64_t cols, int64_t ld, int box_rows);
+
 // channels-last activation (N, H, W, C) fp16 -> 4-D map (C, W, H, N), box (64, bw, bh, bn).
 bool make_map_nhwc(CUtensorMap* m, const void* ptr, int64_t N, int64_t H, int64_t W, int64_t C, int bn, int bh, int bw);
 

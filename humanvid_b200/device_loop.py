@@ -72,6 +72,7 @@ class DeviceDenoiseLoop:
             exchange.prime((self.Bl, self.Cl, self.Fw, self.H, self.W), dev, torch.float16)
         self._graph = None
         self._h = unet._sync_native()
+        self._epoch = unet._epoch   # a rebuilt handle (weights, dtype, FP8 mode) may reuse the old one's address
         N.check(N.lib().hv_set_timestep_source(self._h, C.c_void_p(self.ts.data_ptr()), C.c_void_p(self.step_index.data_ptr())), self._h)
 
     def close(self):
@@ -87,6 +88,7 @@ class DeviceDenoiseLoop:
 
     def matches(self, unet, scheduler, latents, windows, encoder_hidden_states, cond_features, guidance_scale, cfg_on) -> bool:
         return (self._h is not None and unet is self.unet and unet._handle is not None and unet._sync_native().value == self._h.value
+                and unet._epoch == self._epoch
                 and self.exchange is None and tuple(latents.shape) == tuple(self.latents.shape)
                 and [list(w) for w in windows] == self.windows and bool(cfg_on) == self.cfg_on and float(guidance_scale) == self.guidance
                 and [int(t) for t in scheduler._host_timesteps] == self._ts_host and tuple(encoder_hidden_states.shape) == tuple(self.ehs.shape)

@@ -363,6 +363,7 @@ class HvConfig(C.Structure):
         ("clip_layer_norm_eps", C.c_float),
         ("gn_pool_frames", C.c_int32),
         ("no_mid_motion_module", C.c_int32),
+        ("fp8_linears", C.c_int32),
     ]
 
 
@@ -525,7 +526,31 @@ class UNet3DConditionModel(_NativeNet):
         # use_inflated_groupnorm=False: the resnets and conv_norm_out apply nn.GroupNorm to (b, c, f, h, w), pooling over the frames
         cfg.gn_pool_frames = int(not c.use_inflated_groupnorm)
         cfg.no_mid_motion_module = int(self._mm and not c.motion_module_mid_block)
+        cfg.fp8_linears = int(self.__dict__.get("_fp8", False))
         return cfg
+
+    # ---- FP8 mode (DESIGN.md §9) -----------------------------------------------------------------------------------------
+    @property
+    def fp8_linears(self) -> bool:
+        """True while the wide feed-forwards run on e4m3 (enable_fp8_linears)."""
+        return bool(self.__dict__.get("_fp8", False))
+
+    def enable_fp8_linears(self):
+        """Run the LayerNorm -> FF1 -> FF2 chains of the transformers and motion modules of width >= 1280 on e4m3 (per-row weight scales,
+        per-token and per-128 activation scales).  Faster at those widths on an H100, at the cost of the e4m3 quantisation error; the next
+        forward rebuilds the native handle, as a weight change does."""
+        self._set_fp8(True)
+        return self
+
+    def disable_fp8_linears(self):
+        """Back to the fp16 path (the outputs of a model that never enabled FP8)."""
+        self._set_fp8(False)
+        return self
+
+    def _set_fp8(self, on):
+        if self.fp8_linears != bool(on):
+            self.__dict__["_fp8"] = bool(on)
+            self._epoch = getattr(self, "_epoch", 0) + 1
 
     # ---- debug taps (per-layer error ladder; scripts/error_ladder.py) ---------------------------------------------------
     def debug_tap_plan(self, B, F, h, w):

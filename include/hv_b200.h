@@ -85,6 +85,11 @@ typedef struct hv_config {
                                      all F frames of a batch item (nn.GroupNorm on (b, c, f, h, w)); the transformer and motion-module
                                      GroupNorms stay per frame.  A frame's output then depends on the other frames of its window. */
   int32_t no_mid_motion_module;   /* 1: motion_module_mid_block = False -- the mid block has no motion module */
+  /* UNet3DConditionModel only.  0 keeps the fp16 path.  1: FP8 mode (DESIGN.md §9, include/hv_b200_fp8.h): hv_finalize keeps an e4m3 copy of
+     the feed-forward weights of the spatial transformers and motion modules of width >= 1280, and those LayerNorm -> FF1 -> FF2 chains run on
+     e4m3 with per-token / per-128 activation scales (the only covered shapes measured faster than fp16; every other linear stays fp16).
+     Outputs then differ from the fp16 path by the e4m3 quantisation error. */
+  int32_t fp8_linears;
 } hv_config;
 
 int hv_create(const hv_config* cfg, hv_handle* out);
