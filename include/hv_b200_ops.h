@@ -146,8 +146,9 @@ int hv_op_groupnorm_pooled(const void* X, int64_t C1, const void* X2, int64_t C2
                            int64_t NF, int64_t HW, int32_t groups, float eps, int32_t silu, int64_t frames_per_item, float* stats,
                            hv_stream_t stream);
 
-/* LayerNorm over C per row.  Optional: `pre_add` fp16 [rows / rows_per_group][C] is added to x first and the sum is
- * written to `x_out` (the cross-attention residual, see DESIGN.md); `pe` fp16 [F][C] is added to the normalised row
+/* LayerNorm over C per row.  Optional: `pre_add` fp16 [ceil(rows / rows_per_group)][C] (row r adds row r / rows_per_group) is added to
+ * x first and the sum is written to `x_out` (the cross-attention residual, see DESIGN.md; x_out is written only with pre_add; the
+ * statistics use the unrounded fp32 sum); `pe` fp16 [F][C] is added to the normalised row
  * (row -> frame (row / hw) % F) as the motion module does before q/k/v.  HV_ERR_INVALID for: X, gamma, beta or out NULL, any tensor
  * (pre_add, x_out and pe included) not 16-byte aligned, rows < 1, C not a multiple of 8 in [8, 1280], hw or F past INT32_MAX. */
 int hv_op_layernorm(const void* X, const void* gamma, const void* beta, void* out, int64_t rows, int64_t C, float eps,

@@ -26,13 +26,13 @@ pytestmark = pytest.mark.gpu
 
 from conftest import report
 from guarded import Guarded, bits, check_inputs_unchanged
+from norm_bounds import groupnorm_ref_and_bound
 
 if torch.cuda.is_available():
     from humanvid_b200._native import check, i32, i64, lib, ptr, stream
 
 G = 32
 EPS = 1e-5
-U = 2.0 ** -24
 _worst = {}
 
 
@@ -74,55 +74,9 @@ def per_frame(x1, x2, gamma, beta, NF, HW, silu):
     return out
 
 
-def chain_depth(Ct, HW, F):
-    """Longest chain of fp32 additions behind one (item, group) sum, from the launch plan of norm.cu (gn_plan)."""
-    vecs = Ct // 8
-    t = vecs * (1 if vecs >= 256 else 256 // vecs)
-    if t > 1024:
-        t = vecs
-    rpi = t // vecs
-    rpb = max(32, -(-HW // 16))
-    slabs = -(-HW // rpb)
-    cpg = Ct // G
-    rows = -(-rpb // rpi) + 1                      # per-thread row loop, each row adding a (d0 + d1) pair
-    block = rpi * cpg // 2                         # the block's slot loop for one group
-    combine = max(-(-F * slabs // 128) + 7, -(-slabs // 4) + 2)   # finalize (strided loop + tree) or the per-frame 4-lane fold
-    return rows + block + combine
-
-
-def gam(k):
-    return k * U / (1 - k * U)
-
-
 def check_against_fp64(y, x1, x2, gamma, beta, NF, HW, F, silu, label):
     x = torch.cat([x1, x2], -1) if x2 is not None else x1
-    Ct = x.shape[-1]
-    cpg, B, N = Ct // G, NF // F, F * HW * (Ct // G)
-    xd = x.double().view(B, F, HW, G, cpg)
-    p = xd[:, 0, 0, :, 0]                                              # (B, G) the kernel's pivot
-    d = xd - p[:, None, None, :, None]
-    A, Q = d.abs().sum((1, 2, 4)) / N, (d * d).sum((1, 2, 4)) / N      # per (item, group), divided by N
-    mp = d.sum((1, 2, 4)) / N
-    del d
-    mean = p + mp
-    var = (Q - mp * mp).clamp_min(0)
-    rstd = 1.0 / torch.sqrt(var + EPS)
-    D = chain_depth(Ct, HW, F)
-    e_mp = gam(D + 1) * A + 2 * U * mp.abs()
-    e_mean = e_mp + U * mean.abs()
-    e_var = gam(D + 3) * Q + 2 * mp.abs() * e_mp + e_mp ** 2 + 4 * U * (Q + mp * mp)
-    rel_rstd = e_var / (2 * (var + EPS)) * (1 + e_var / (var + EPS)) + 2.0 ** -22 + U
-    gm, bt = gamma.double().view(G, cpg), beta.double().view(G, cpg)
-    bc = lambda t: t[:, None, None, :, None]
-    sc = bc(rstd) * gm
-    sh = bt - bc(mean) * sc
-    yr = (xd - bc(mean)) * sc + bt
-    dy = (xd - bc(mean)).abs() * gm.abs() * bc(rstd) * (bc(rel_rstd) + U) + sc.abs() * bc(e_mean) + U * (sh.abs() + yr.abs())
-    if silu:
-        s = yr * torch.sigmoid(yr)
-        dy = 1.1 * dy + (5 + 1.2 * yr.abs()) * 2.0 ** -23 * s.abs()
-        yr = s
-    bound = 2.0 ** -11 * (yr.abs() + dy) + dy + 2.0 ** -25
+    yr, bound = groupnorm_ref_and_bound(x.view(NF, HW, -1), gamma, beta, F, G, EPS, silu)
     err = (y.double().view_as(yr) - yr).abs()
     ratio = float((err / bound).max())
     relL2 = float((y.double().view_as(yr) - yr).norm() / yr.norm())
