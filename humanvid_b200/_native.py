@@ -30,6 +30,9 @@ class Epilogue(C.Structure):
 
 ACT_NONE, ACT_RELU, ACT_SILU, ACT_QUICK_GELU = 0, 1, 2, 3
 
+# enum hv_kind in include/hv_b200.h: hv_config.kind, the network a handle runs
+HV_KIND_UNET3D, HV_KIND_POSE_GUIDER, HV_KIND_CAMERA_ENCODER, HV_KIND_UNET2D_REF, HV_KIND_VAE, HV_KIND_CLIP_VISION = 0, 1, 2, 3, 4, 5
+
 
 def lib() -> C.CDLL:
     global _lib
@@ -40,13 +43,12 @@ def lib() -> C.CDLL:
                 "(humanvid_b200 has no non-CUDA fallback)"
             )
         _lib = C.CDLL(LIB_PATH)
+        # the entry points Python calls that do not return int
         _lib.hv_ops_last_error.restype = C.c_char_p
-        try:
-            _lib.hv_last_error.restype = C.c_char_p
-            _lib.hv_last_error.argtypes = [C.c_void_p]
-            _lib.hv_workspace_bytes.restype = C.c_size_t
-        except AttributeError:
-            pass
+        _lib.hv_last_error.restype = C.c_char_p
+        _lib.hv_last_error.argtypes = [C.c_void_p]
+        _lib.hv_workspace_bytes.restype = C.c_size_t
+        _lib.hv_last_launch_count.restype = C.c_int64
     return _lib
 
 

@@ -22,6 +22,7 @@ CPU fallback: without the library, or on a non-CUDA tensor, ``forward`` raises.
 from __future__ import annotations
 
 import ctypes as C
+import inspect
 import json
 import math
 import os
@@ -185,6 +186,14 @@ class _Sampler(_Shell):
         self.conv = _conv(ch, ch, 3, stride=stride, padding=1)
 
 
+def _torch_dfs(m):
+    """Every module under `m` in pre-order, like the reference's torch_dfs (mutual_self_attention.py): no deduplication."""
+    out = [m]
+    for c in m.children():
+        out += _torch_dfs(c)
+    return out
+
+
 class _Block(_Shell):
     def __init__(self, res_io, ch, attn, motion, xdim, temb, groups, max_len, sampler=None, block_cls=None):
         super().__init__()
@@ -206,6 +215,91 @@ class _TimestepEmbedding(_Shell):
         self.linear_2 = nn.Linear(cout, cout)
 
 
+def _sd15_unsupported(c, dim):
+    """The SD1.5 layout checks both UNets share, on config `c`; `dim` ("2D" / "3D") ends the block type names."""
+    unsupported = []
+    if tuple(c.down_block_types) != (f"CrossAttnDownBlock{dim}",) * 3 + (f"DownBlock{dim}",) \
+            or tuple(c.up_block_types) != (f"UpBlock{dim}",) + (f"CrossAttnUpBlock{dim}",) * 3:
+        unsupported.append("block types other than the SD1.5 layout")
+    if c.layers_per_block != 2 or len(c.block_out_channels) != 4:
+        unsupported.append("layers_per_block != 2 / depth != 4")
+    if c.center_input_sample or not c.flip_sin_to_cos or c.freq_shift != 0 or c.use_linear_projection or c.dual_cross_attention:
+        unsupported.append("center_input_sample / flip_sin_to_cos=False / freq_shift / use_linear_projection / dual_cross_attention")
+    if c.class_embed_type is not None or c.num_class_embeds is not None:
+        unsupported.append("class embeddings")
+    if c.resnet_time_scale_shift != "default" or c.act_fn not in ("silu", "swish") or c.mid_block_scale_factor != 1 \
+            or not isinstance(c.attention_head_dim, int):
+        unsupported.append("non-default resnet/act options")
+    return unsupported
+
+
+def _build_sd15_unet(unet, in_channels, ch, xdim, groups, motion=False, mid_motion=False, max_len=0, block_cls=None):
+    """conv_in, time_embedding and the down / mid / up ``_Block`` tree of the SD1.5 layout on `unet`.  ``block_cls=None`` builds the
+    denoising UNet's blocks, each with ``motion_modules`` (motion modules where `motion` / `mid_motion`, else None entries); the writer UNet
+    passes its ``BasicTransformerBlock``.  down_blocks and up_blocks are registered before mid_block: the module walk, and so the bank
+    order, is down, up, mid as in the reference."""
+    temb = ch[0] * 4
+    unet.conv_in = _conv(in_channels, ch[0], 3, padding=1)
+    unet.time_embedding = _TimestepEmbedding(ch[0], temb)
+    unet.down_blocks = nn.ModuleList([])
+    unet.up_blocks = nn.ModuleList([])
+    prev = ch[0]
+    for i, c in enumerate(ch):
+        last = i == 3
+        unet.down_blocks.append(_Block([(prev, c), (c, c)], c, 0 if last else 2, motion, xdim, temb, groups, max_len, None if last else "down", block_cls))
+        prev = c
+    unet.mid_block = _Block([(ch[3], ch[3]), (ch[3], ch[3])], ch[3], 1, mid_motion, xdim, temb, groups, max_len, "mid", block_cls)
+    rev = ch[::-1]
+    prev = rev[0]
+    for i, c in enumerate(rev):
+        cin = rev[min(i + 1, 3)]
+        io = [((prev if j == 0 else c) + (cin if j == 2 else c), c) for j in range(3)]
+        unet.up_blocks.append(_Block(io, c, 0 if i == 0 else 3, motion, xdim, temb, groups, max_len, "up" if i < 3 else None, block_cls))
+        prev = c
+
+
+def _sd15_hv_config(c, kind):
+    """The HvConfig fields both UNets fill from their config."""
+    cfg = HvConfig()
+    cfg.kind = kind
+    cfg.in_channels, cfg.out_channels = c.in_channels, c.out_channels
+    cfg.block_out_channels = (C.c_int32 * 4)(*c.block_out_channels)
+    cfg.heads, cfg.cross_attention_dim, cfg.norm_groups = c.attention_head_dim, c.cross_attention_dim, c.norm_num_groups
+    return cfg
+
+
+def _read_state(path):
+    """A checkpoint file's state dict on the CPU: safetensors by suffix, else a torch pickle of tensors."""
+    if os.path.splitext(path)[1].lower() == ".safetensors":
+        from safetensors.torch import load_file
+
+        return load_file(path, device="cpu")
+    return torch.load(path, map_location="cpu", weights_only=True)
+
+
+def _from_pretrained(cls, pretrained_model_path, subfolder=None, overrides=None, weights=("diffusion_pytorch_model.safetensors",
+                     "diffusion_pytorch_model.bin"), require_all=False, torch_dtype=None):
+    """``<path>[/<subfolder>]/config.json`` without its ``_`` keys -> ``cls`` from the keywords its ``__init__`` takes, then `overrides`;
+    weights from ``weights[0]`` (safetensors) or else ``weights[1]``, loaded with strict=False.  With `require_all`, a parameter the
+    checkpoint lacks raises.  Builds on the CPU."""
+    path = os.path.join(str(pretrained_model_path), subfolder) if subfolder is not None else str(pretrained_model_path)
+    with open(os.path.join(path, "config.json")) as f:
+        cfg = {k: v for k, v in json.load(f).items() if not k.startswith("_")}
+    allowed = set(inspect.signature(cls.__init__).parameters) - {"self", "unused"}
+    model = cls(**{**{k: v for k, v in cfg.items() if k in allowed}, **(overrides or {})})
+    st_path, bin_path = (os.path.join(path, w) for w in weights)
+    if os.path.exists(st_path):
+        state = _read_state(st_path)
+    elif os.path.isfile(bin_path):
+        state = _read_state(bin_path)
+    else:
+        raise FileNotFoundError(f"no weights file found in {path}")
+    missing = model.load_state_dict(state, strict=False).missing_keys
+    if require_all and missing:
+        raise RuntimeError(f"{path}: weights missing from the checkpoint: {missing[:5]}{' ...' if len(missing) > 5 else ''}")
+    return model.to(torch_dtype) if torch_dtype is not None else model
+
+
 @dataclass
 class UNet3DConditionOutput:
     sample: torch.Tensor
@@ -214,8 +308,6 @@ class UNet3DConditionOutput:
 # --------------------------------------------------------------------------------------------- native base
 class _NativeNet(nn.Module):
     """Owns one ``hv_handle``; pushes the module's state_dict into it whenever parameters changed."""
-
-    _kind = 0
 
     def __init__(self):
         super().__init__()
@@ -283,6 +375,16 @@ class _NativeNet(nn.Module):
             N.check(N.lib().hv_reserve_workspace(h, N.i32(B), N.i32(F), N.i32(H), N.i32(W)), h)
             self._reserved.add(key)
 
+    def _workspace_bytes(self, B, F, H, W) -> int:
+        hd = self._sync_native()
+        return int(N.lib().hv_workspace_bytes(hd, N.i32(B), N.i32(F), N.i32(H), N.i32(W)))
+
+    def _run(self, entry, h, shape, *args):
+        """Reserve the workspace for `shape` (``_reserve``'s B, F, H, W[, variant]), call the C forward `entry` as
+        ``entry(h, *args, NULL workspace, 0, current stream)`` and raise with the handle's message on a non-zero status."""
+        self._reserve(h, *shape)
+        N.check(entry(h, *args, None, C.c_size_t(0), N.stream()), h)
+
     def __del__(self):
         try:
             self._destroy()
@@ -323,13 +425,16 @@ class _NativeNet(nn.Module):
             raise RuntimeError(f"{what} must be a CUDA tensor (humanvid_b200 has no CPU path)")
         return x.to(torch.float16).contiguous()
 
+    @staticmethod
+    def _from_half(t: torch.Tensor, dtype: torch.dtype) -> torch.Tensor:
+        """A forward's fp16 result in the caller's dtype."""
+        return t if dtype == torch.float16 else t.to(dtype)
+
     @property
     def last_launch_count(self) -> int:
         if self._handle is None:
             return 0
-        f = N.lib().hv_last_launch_count
-        f.restype = C.c_int64
-        return int(f(self._handle))
+        return int(N.lib().hv_last_launch_count(self._handle))
 
 
 class HvConfig(C.Structure):
@@ -371,8 +476,6 @@ class HvConfig(C.Structure):
 class UNet3DConditionModel(_NativeNet):
     """Drop-in for src/models/unet_3d.py:30-577 (inference): same ctor keywords, forward signature, state_dict keys."""
 
-    _kind = 0
-
     def __init__(
         self,
         sample_size: Optional[int] = None,
@@ -411,18 +514,11 @@ class UNet3DConditionModel(_NativeNet):
         unet_use_temporal_attention=None,
     ):
         super().__init__()
+        self.config = SimpleNamespace(**{k: v for k, v in locals().items() if k not in ("self", "__class__")})
         mmk = dict(motion_module_kwargs or {})
-        unsupported = []
-        if tuple(down_block_types) != ("CrossAttnDownBlock3D",) * 3 + ("DownBlock3D",) or tuple(up_block_types) != ("UpBlock3D",) + ("CrossAttnUpBlock3D",) * 3:
-            unsupported.append("block types other than the SD1.5 layout")
-        if layers_per_block != 2 or len(block_out_channels) != 4:
-            unsupported.append("layers_per_block != 2 / depth != 4")
-        if center_input_sample or not flip_sin_to_cos or freq_shift != 0 or use_linear_projection or dual_cross_attention:
-            unsupported.append("center_input_sample / flip_sin_to_cos=False / freq_shift / use_linear_projection / dual_cross_attention")
-        if class_embed_type is not None or num_class_embeds is not None or unet_use_temporal_attention or unet_use_cross_frame_attention:
-            unsupported.append("class embeddings / unet_use_temporal_attention / cross_frame_attention")
-        if resnet_time_scale_shift != "default" or act_fn not in ("silu", "swish") or mid_block_scale_factor != 1 or not isinstance(attention_head_dim, int):
-            unsupported.append("non-default resnet/act options")
+        unsupported = _sd15_unsupported(self.config, "3D")
+        if unet_use_temporal_attention or unet_use_cross_frame_attention:
+            unsupported.append("unet_use_temporal_attention / cross_frame_attention")
         if use_motion_module and (
             tuple(motion_module_resolutions) != (1, 2, 4, 8) or motion_module_decoder_only
             or motion_module_type != "Vanilla" or mmk.get("num_transformer_block", 1) != 1
@@ -433,35 +529,14 @@ class UNet3DConditionModel(_NativeNet):
         if unsupported:
             raise NotImplementedError("humanvid_b200.UNet3DConditionModel implements the inference_v1 / inference_v2 hot path only; unsupported: "
                                       + "; ".join(unsupported))
-        self.config = SimpleNamespace(**{k: v for k, v in locals().items() if k not in ("self", "mmk", "unsupported", "__class__")})
         self.sample_size = sample_size
         self.in_channels = in_channels
         ch = list(block_out_channels)
-        heads, xdim, g = attention_head_dim, cross_attention_dim, norm_num_groups
-        temb = ch[0] * 4
-        mm = bool(use_motion_module)
-        max_len = mmk.get("temporal_position_encoding_max_len", 24)
-        self._heads, self._max_len, self._mm = heads, max_len, mm
-        mid_mm = mm and bool(motion_module_mid_block)   # inference_v1.yaml: no motion module in the mid block
-        self.conv_in = _conv(in_channels, ch[0], 3, padding=1)
-        self.time_embedding = _TimestepEmbedding(ch[0], temb)
-        self.down_blocks = nn.ModuleList([])
-        self.mid_block = None
-        self.up_blocks = nn.ModuleList([])
-        prev = ch[0]
-        for i, c in enumerate(ch):
-            last = i == 3
-            self.down_blocks.append(_Block([(prev, c), (c, c)], c, 0 if last else 2, mm, xdim, temb, g, max_len, None if last else "down"))
-            prev = c
-        self.mid_block = _Block([(ch[3], ch[3]), (ch[3], ch[3])], ch[3], 1, mid_mm, xdim, temb, g, max_len, "mid")
-        rev = ch[::-1]
-        prev = rev[0]
-        for i, c in enumerate(rev):
-            cin = rev[min(i + 1, 3)]
-            io = [((prev if j == 0 else c) + (cin if j == 2 else c), c) for j in range(3)]
-            self.up_blocks.append(_Block(io, c, 0 if i == 0 else 3, mm, xdim, temb, g, max_len, "up" if i < 3 else None))
-            prev = c
-        self.conv_norm_out = nn.GroupNorm(g, ch[0], eps=norm_eps)
+        self._mm = mm = bool(use_motion_module)
+        self._max_len = mmk.get("temporal_position_encoding_max_len", 24)
+        # inference_v1.yaml: no motion module in the mid block
+        _build_sd15_unet(self, in_channels, ch, cross_attention_dim, norm_num_groups, mm, mm and bool(motion_module_mid_block), self._max_len)
+        self.conv_norm_out = nn.GroupNorm(norm_num_groups, ch[0], eps=norm_eps)
         self.conv_out = _conv(ch[0], out_channels, 3, padding=1)
         self._ref_cfg = True
         self._forward_flags = None   # humanvid_b200.distributed sets HV_FLAG_UNCOND_ONLY / HV_FLAG_COND_ONLY for one-half units
@@ -469,16 +544,9 @@ class UNet3DConditionModel(_NativeNet):
     # ---- reference banks (ReferenceAttentionControl, read side) -----------------------------------------------
     def reader_blocks(self) -> List[TemporalBasicTransformerBlock]:
         """fusion_blocks='full' order of mutual_self_attention.py:284-300."""
-
-        def dfs(m):
-            out = [m]
-            for c in m.children():
-                out += dfs(c)
-            return out
-
         cached = self.__dict__.get("_reader_blocks_cache")
         if cached is None:      # the module tree is fixed after __init__: walk it once (1 ms per forward otherwise)
-            mods = [m for m in dfs(self) if isinstance(m, TemporalBasicTransformerBlock)]
+            mods = [m for m in _torch_dfs(self) if isinstance(m, TemporalBasicTransformerBlock)]
             cached = sorted(mods, key=lambda m: -m.norm1.normalized_shape[0])
             self.__dict__["_reader_blocks_cache"] = cached
         return list(cached)
@@ -517,11 +585,7 @@ class UNet3DConditionModel(_NativeNet):
 
     def _hv_config(self):
         c = self.config
-        cfg = HvConfig()
-        cfg.kind = 0
-        cfg.in_channels, cfg.out_channels = c.in_channels, c.out_channels
-        cfg.block_out_channels = (C.c_int32 * 4)(*c.block_out_channels)
-        cfg.heads, cfg.cross_attention_dim, cfg.norm_groups = c.attention_head_dim, c.cross_attention_dim, c.norm_num_groups
+        cfg = _sd15_hv_config(c, N.HV_KIND_UNET3D)
         cfg.use_motion_module, cfg.motion_max_len = int(self._mm), self._max_len
         # use_inflated_groupnorm=False: the resnets and conv_norm_out apply nn.GroupNorm to (b, c, f, h, w), pooling over the frames
         cfg.gn_pool_frames = int(not c.use_inflated_groupnorm)
@@ -576,10 +640,7 @@ class UNet3DConditionModel(_NativeNet):
         N.check(N.lib().hv_debug_set_taps(hd, arr if tensors else None, N.i32(len(tensors))), hd)
 
     def workspace_bytes(self, B, F, h, w) -> int:
-        hd = self._sync_native()
-        f = N.lib().hv_workspace_bytes
-        f.restype = C.c_size_t
-        return int(f(hd, N.i32(B), N.i32(F), N.i32(h), N.i32(w)))
+        return self._workspace_bytes(B, F, h, w)
 
     @torch.no_grad()
     def forward(
@@ -613,10 +674,10 @@ class UNet3DConditionModel(_NativeNet):
         t = int(timestep.reshape(-1)[0].item()) if torch.is_tensor(timestep) else int(timestep)
         out = torch.empty((B, self.config.out_channels, F, H, W), device=x.device, dtype=torch.float16)
         flags = self._forward_flags if self._forward_flags is not None else (1 if self._ref_cfg else 0)
-        self._reserve(h, B, F, H, W, tuple(tuple(t.shape) for t in (self._bank_refs or ())))   # the banks' K/V scratch is planned too
-        N.check(N.lib().hv_unet3d_forward(h, N.ptr(x), N.i64(t), N.ptr(ehs), N.ptr(pose), N.ptr(out), N.i32(B), N.i32(F), N.i32(H), N.i32(W),
-                                          C.c_uint32(flags), None, C.c_size_t(0), N.stream()), h)
-        out = out.to(sample.dtype) if sample.dtype != torch.float16 else out
+        banks = tuple(tuple(t.shape) for t in (self._bank_refs or ()))   # the banks' K/V scratch is planned too
+        self._run(N.lib().hv_unet3d_forward, h, (B, F, H, W, banks), N.ptr(x), N.i64(t), N.ptr(ehs), N.ptr(pose), N.ptr(out), N.i32(B), N.i32(F),
+                  N.i32(H), N.i32(W), C.c_uint32(flags))
+        out = self._from_half(out, sample.dtype)
         if not return_dict:
             return (out,)
         return UNet3DConditionOutput(sample=out)
@@ -624,47 +685,22 @@ class UNet3DConditionModel(_NativeNet):
     # ---- loading (unet_3d.py:579-670) ---------------------------------------------------------------------------
     @classmethod
     def from_pretrained_2d(cls, pretrained_model_path, motion_module_path, subfolder=None, unet_additional_kwargs=None, mm_zero_proj_out=False):
-        path = os.path.join(str(pretrained_model_path), subfolder) if subfolder is not None else str(pretrained_model_path)
-        config_file = os.path.join(path, "config.json")
-        if not (os.path.exists(config_file) and os.path.isfile(config_file)):
+        config_file = os.path.join(str(pretrained_model_path), subfolder or "", "config.json")
+        if not os.path.isfile(config_file):
             raise RuntimeError(f"{config_file} does not exist or is not a file")
-        with open(config_file) as f:
-            cfg = json.load(f)
-        cfg = {k: v for k, v in cfg.items() if not k.startswith("_")}
-        cfg["down_block_types"] = ["CrossAttnDownBlock3D"] * 3 + ["DownBlock3D"]
-        cfg["up_block_types"] = ["UpBlock3D"] + ["CrossAttnUpBlock3D"] * 3
-        cfg["mid_block_type"] = "UNetMidBlock3DCrossAttn"
-        import inspect
-
-        allowed = set(inspect.signature(cls.__init__).parameters)
-        kw = {k: v for k, v in cfg.items() if k in allowed}
-        kw.update(unet_additional_kwargs or {})
-        model = cls(**kw)
-        st_path = os.path.join(path, "diffusion_pytorch_model.safetensors")
-        if os.path.exists(st_path):
-            from safetensors.torch import load_file
-
-            state = load_file(st_path, device="cpu")
-        else:
-            bin_path = os.path.join(path, "diffusion_pytorch_model.bin")
-            if not os.path.isfile(bin_path):
-                raise FileNotFoundError(f"no weights file found in {path}")
-            state = torch.load(bin_path, map_location="cpu", weights_only=True)
+        blocks = dict(down_block_types=["CrossAttnDownBlock3D"] * 3 + ["DownBlock3D"], up_block_types=["UpBlock3D"] + ["CrossAttnUpBlock3D"] * 3,
+                      mid_block_type="UNetMidBlock3DCrossAttn")
+        model = _from_pretrained(cls, pretrained_model_path, subfolder, {**blocks, **(unet_additional_kwargs or {})})
         mp = str(motion_module_path)
-        if os.path.exists(mp) and os.path.isfile(mp):
+        if os.path.isfile(mp):
             suffix = os.path.splitext(mp)[1].lower()
-            if suffix in (".pth", ".pt", ".ckpt"):
-                mm_state = torch.load(mp, map_location="cpu", weights_only=True)
-            elif suffix == ".safetensors":
-                from safetensors.torch import load_file
-
-                mm_state = load_file(mp, device="cpu")
-            else:
+            if suffix not in (".pth", ".pt", ".ckpt", ".safetensors"):
                 raise RuntimeError(f"unknown file format for motion module weights: {suffix}")
+            mm_state = _read_state(mp)
             if mm_zero_proj_out:
                 mm_state = {k: v for k, v in mm_state.items() if "proj_out" not in k}
-            state.update(mm_state)   # every key, like the reference (unet_3d.py:657-658); load_state_dict(strict=False) drops what the model lacks
-        model.load_state_dict(state, strict=False)
+            # every key, like the reference (unet_3d.py:657-658): one the 2-D file also has is overwritten, one the model lacks is dropped
+            model.load_state_dict(mm_state, strict=False)
         return model
 
 # --------------------------------------------------------------------------------------------- reference ("writer") UNet
@@ -682,8 +718,6 @@ class UNet2DConditionModel(_NativeNet):
     is left in ``block.bank`` (mutual_self_attention.py:137-146), ready for ``reader.update(writer)``.  The native forward
     (``hv_unet2d_reference_forward``) is the denoising UNet's own kernels at one frame without motion modules.
     """
-
-    _kind = 3
 
     def __init__(
         self,
@@ -715,43 +749,15 @@ class UNet2DConditionModel(_NativeNet):
         **unused,
     ):
         super().__init__()
-        unsupported = []
-        if tuple(down_block_types) != ("CrossAttnDownBlock2D",) * 3 + ("DownBlock2D",) or tuple(up_block_types) != ("UpBlock2D",) + ("CrossAttnUpBlock2D",) * 3 \
-                or mid_block_type != "UNetMidBlock2DCrossAttn":
-            unsupported.append("block types other than the SD1.5 layout")
-        if layers_per_block != 2 or len(block_out_channels) != 4:
-            unsupported.append("layers_per_block != 2 / depth != 4")
-        if center_input_sample or not flip_sin_to_cos or freq_shift != 0 or use_linear_projection or dual_cross_attention or only_cross_attention:
-            unsupported.append("center_input_sample / flip_sin_to_cos=False / freq_shift / use_linear_projection / dual / only_cross_attention")
-        if class_embed_type is not None or num_class_embeds is not None or resnet_time_scale_shift != "default" or act_fn not in ("silu", "swish") \
-                or mid_block_scale_factor != 1 or not isinstance(attention_head_dim, int) or norm_num_groups is None:
-            unsupported.append("class embeddings / non-default resnet, activation or norm options")
+        self.config = SimpleNamespace(**{k: v for k, v in locals().items() if k not in ("self", "unused", "__class__")})
+        unsupported = _sd15_unsupported(self.config, "2D")
+        if mid_block_type != "UNetMidBlock2DCrossAttn" or only_cross_attention or norm_num_groups is None:
+            unsupported.append("mid_block_type / only_cross_attention / norm_num_groups=None")
         if unsupported:
             raise NotImplementedError("humanvid_b200.UNet2DConditionModel implements the SD1.5 reference-UNet layout only; unsupported: " + "; ".join(unsupported))
-        self.config = SimpleNamespace(**{k: v for k, v in locals().items() if k not in ("self", "unsupported", "unused", "__class__")})
         self.sample_size = sample_size
         self.in_channels = in_channels
-        ch = list(block_out_channels)
-        heads, xdim, g = attention_head_dim, cross_attention_dim, norm_num_groups
-        temb = ch[0] * 4
-        self._heads = heads
-        self.conv_in = _conv(in_channels, ch[0], 3, padding=1)
-        self.time_embedding = _TimestepEmbedding(ch[0], temb)
-        self.down_blocks = nn.ModuleList([])
-        self.up_blocks = nn.ModuleList([])
-        prev = ch[0]
-        for i, c in enumerate(ch):
-            last = i == 3
-            self.down_blocks.append(_Block([(prev, c), (c, c)], c, 0 if last else 2, False, xdim, temb, g, 0, None if last else "down", block_cls=BasicTransformerBlock))
-            prev = c
-        self.mid_block = _Block([(ch[3], ch[3]), (ch[3], ch[3])], ch[3], 1, False, xdim, temb, g, 0, "mid", block_cls=BasicTransformerBlock)
-        rev = ch[::-1]
-        prev = rev[0]
-        for i, c in enumerate(rev):
-            cin = rev[min(i + 1, 3)]
-            io = [((prev if j == 0 else c) + (cin if j == 2 else c), c) for j in range(3)]
-            self.up_blocks.append(_Block(io, c, 0 if i == 0 else 3, False, xdim, temb, g, 0, "up" if i < 3 else None, block_cls=BasicTransformerBlock))
-            prev = c
+        _build_sd15_unet(self, in_channels, list(block_out_channels), cross_attention_dim, norm_num_groups, block_cls=BasicTransformerBlock)
         self._ref_write = False
 
     # ---- banks (ReferenceAttentionControl, write side) ---------------------------------------------------------
@@ -768,14 +774,7 @@ class UNet2DConditionModel(_NativeNet):
         return sorted(out, key=lambda t: -t[0].norm1.normalized_shape[0])
 
     def _hv_config(self):
-        c = self.config
-        cfg = HvConfig()
-        cfg.kind = 3
-        cfg.in_channels, cfg.out_channels = c.in_channels, c.out_channels
-        cfg.block_out_channels = (C.c_int32 * 4)(*c.block_out_channels)
-        cfg.heads, cfg.cross_attention_dim, cfg.norm_groups = c.attention_head_dim, c.cross_attention_dim, c.norm_num_groups
-        cfg.use_motion_module, cfg.motion_max_len = 0, 0
-        return cfg
+        return _sd15_hv_config(self.config, N.HV_KIND_UNET2D_REF)
 
     @torch.no_grad()
     def forward(self, sample: torch.Tensor, timestep: Union[torch.Tensor, float, int], encoder_hidden_states: torch.Tensor,
@@ -800,13 +799,12 @@ class UNet2DConditionModel(_NativeNet):
         banks = [torch.empty((B, (H >> lvl) * (W >> lvl), blk.norm1.normalized_shape[0]), device=x.device, dtype=torch.float16) for blk, lvl in blocks]
         hidden = torch.empty((B, self.config.block_out_channels[0], H, W), device=x.device, dtype=torch.float16)
         ptrs = (C.c_void_p * len(banks))(*[b.data_ptr() for b in banks])
-        self._reserve(h, B, 1, H, W)
-        N.check(N.lib().hv_unet2d_reference_forward(h, N.ptr(x), N.i64(t), N.ptr(ehs), N.ptr(hidden), ptrs, N.i32(len(banks)), N.i32(B), N.i32(H), N.i32(W),
-                                                    None, C.c_size_t(0), N.stream()), h)
+        self._run(N.lib().hv_unet2d_reference_forward, h, (B, 1, H, W), N.ptr(x), N.i64(t), N.ptr(ehs), N.ptr(hidden), ptrs, N.i32(len(banks)),
+                  N.i32(B), N.i32(H), N.i32(W))
         if self._ref_write:
             for (blk, _), bank in zip(blocks, banks):
                 blk.bank.append(bank)
-        hidden = hidden.to(sample.dtype) if sample.dtype != torch.float16 else hidden
+        hidden = self._from_half(hidden, sample.dtype)
         if not return_dict:
             return (hidden,)
         return UNet2DConditionOutput(sample=hidden)
@@ -814,22 +812,7 @@ class UNet2DConditionModel(_NativeNet):
     @classmethod
     def from_pretrained(cls, pretrained_model_path, subfolder=None, **kwargs):
         """diffusers-style loader (scripts/pose2vid.py:72-75): ``<path>/<subfolder>/config.json`` + ``diffusion_pytorch_model.{safetensors,bin}``."""
-        path = os.path.join(str(pretrained_model_path), subfolder) if subfolder is not None else str(pretrained_model_path)
-        with open(os.path.join(path, "config.json")) as f:
-            cfg = {k: v for k, v in json.load(f).items() if not k.startswith("_")}
-        import inspect
-
-        allowed = set(inspect.signature(cls.__init__).parameters) - {"self", "unused"}
-        model = cls(**{k: v for k, v in cfg.items() if k in allowed})
-        st_path = os.path.join(path, "diffusion_pytorch_model.safetensors")
-        if os.path.exists(st_path):
-            from safetensors.torch import load_file
-
-            state = load_file(st_path, device="cpu")
-        else:
-            state = torch.load(os.path.join(path, "diffusion_pytorch_model.bin"), map_location="cpu", weights_only=True)
-        model.load_state_dict(state, strict=False)   # SD checkpoints also carry conv_norm_out / conv_out, unused by the reference UNet
-        return model
+        return _from_pretrained(cls, pretrained_model_path, subfolder)   # SD checkpoints also carry conv_norm_out / conv_out, unused by the reference UNet
 
 
 # --------------------------------------------------------------------------------------------- PoseGuider
@@ -854,7 +837,7 @@ class PoseGuider(_NativeNet):
     def _hv_config(self):
         out, cin, ch = self._cfg
         cfg = HvConfig()
-        cfg.kind = 1
+        cfg.kind = N.HV_KIND_POSE_GUIDER
         cfg.pg_cond_channels, cfg.pg_out_channels = cin, out
         cfg.pg_block_channels = (C.c_int32 * 4)(*ch)
         cfg.norm_groups = 32
@@ -868,9 +851,8 @@ class PoseGuider(_NativeNet):
         h = self._sync_native()
         x = self._as_half(conditioning, "conditioning")
         out = torch.empty((B, self._cfg[0], F, H // 8, W // 8), device=x.device, dtype=torch.float16)
-        self._reserve(h, B, F, H, W)
-        N.check(N.lib().hv_pose_guider_forward(h, N.ptr(x), N.ptr(out), N.i32(B), N.i32(F), N.i32(H), N.i32(W), None, C.c_size_t(0), N.stream()), h)
-        return out.to(conditioning.dtype) if conditioning.dtype != torch.float16 else out
+        self._run(N.lib().hv_pose_guider_forward, h, (B, F, H, W), N.ptr(x), N.ptr(out), N.i32(B), N.i32(F), N.i32(H), N.i32(W))
+        return self._from_half(out, conditioning.dtype)
 
 
 # --------------------------------------------------------------------------------------------- CameraPoseEncoder
@@ -914,7 +896,7 @@ class CameraPoseEncoder(_NativeNet):
     def _hv_config(self):
         d = self._cfg
         cfg = HvConfig()
-        cfg.kind = 2
+        cfg.kind = N.HV_KIND_CAMERA_ENCODER
         cfg.cam_downscale, cfg.cam_cin, cfg.cam_channels = d["downscale"], d["cin"], d["c"]
         cfg.cam_nums_rb, cfg.cam_heads, cfg.cam_max_len = d["nums_rb"], d["heads"], d["max_len"]
         cfg.heads = d["heads"]
@@ -932,9 +914,8 @@ class CameraPoseEncoder(_NativeNet):
         h = self._sync_native()
         xin = self._as_half(x, "plucker embedding")
         out = torch.empty((B * F, self._cfg["c"], H // r, W // r), device=xin.device, dtype=torch.float16)
-        self._reserve(h, B, F, H, W)
-        N.check(N.lib().hv_camera_encoder_forward(h, N.ptr(xin), N.ptr(out), N.i32(B), N.i32(F), N.i32(H), N.i32(W), None, C.c_size_t(0), N.stream()), h)
-        return [out.to(x.dtype) if x.dtype != torch.float16 else out]
+        self._run(N.lib().hv_camera_encoder_forward, h, (B, F, H, W), N.ptr(xin), N.ptr(out), N.i32(B), N.i32(F), N.i32(H), N.i32(W))
+        return [self._from_half(out, x.dtype)]
 
 
     @torch.no_grad()
@@ -952,10 +933,9 @@ class CameraPoseEncoder(_NativeNet):
         K = intrinsics.to(dev, torch.float32).contiguous()
         M = c2w.to(dev, torch.float32).contiguous()
         out = torch.empty((B * F, self._cfg["c"], height // r, width // r), device=dev, dtype=torch.float16)
-        self._reserve(h, B, F, height, width)
-        N.check(N.lib().hv_camera_encoder_forward_rays(h, N.ptr(K), N.ptr(M), N.ptr(out), N.i32(B), N.i32(F), N.i32(height), N.i32(width), None,
-                                                       C.c_size_t(0), N.stream()), h)
-        return [out.to(self.dtype) if self.dtype != torch.float16 else out]
+        self._run(N.lib().hv_camera_encoder_forward_rays, h, (B, F, height, width), N.ptr(K), N.ptr(M), N.ptr(out), N.i32(B), N.i32(F),
+                  N.i32(height), N.i32(width))
+        return [self._from_half(out, self.dtype)]
 
 
 # --------------------------------------------------------------------------------------------- ReferenceAttentionControl (reader)
@@ -998,14 +978,7 @@ class ReferenceAttentionControl:
         root = writer.unet if hasattr(writer, "unet") else writer
         if isinstance(root, UNet2DConditionModel):
             return [m for m, _ in root.writer_blocks()]
-
-        def dfs(m):
-            out = [m]
-            for c in m.children():
-                out += dfs(c)
-            return out
-
-        mods = [m for m in dfs(root) if hasattr(m, "bank") and hasattr(m, "norm1") and hasattr(m, "attn1")]
+        mods = [m for m in _torch_dfs(root) if hasattr(m, "bank") and hasattr(m, "norm1") and hasattr(m, "attn1")]
         return sorted(mods, key=lambda m: -m.norm1.normalized_shape[0])
 
     def update(self, writer, dtype=torch.float16):
@@ -1151,8 +1124,6 @@ class AutoencoderKL(_NativeNet):
     the others.  Inference only: no tiling / slicing, no ``latent_dist.sample()``.
     """
 
-    _kind = 4
-
     def __init__(
         self,
         in_channels: int = 3,
@@ -1201,7 +1172,7 @@ class AutoencoderKL(_NativeNet):
     def _hv_config(self):
         c = self.config
         cfg = HvConfig()
-        cfg.kind = 4
+        cfg.kind = N.HV_KIND_VAE
         cfg.in_channels, cfg.out_channels = c.in_channels, c.out_channels
         cfg.block_out_channels = (C.c_int32 * 4)(*c.block_out_channels)
         cfg.norm_groups = c.norm_num_groups
@@ -1214,10 +1185,7 @@ class AutoencoderKL(_NativeNet):
 
     def workspace_bytes(self, n, h, w) -> int:
         """Device workspace of decoding n latents of h x w and of encoding n images of 8h x 8w."""
-        hd = self._sync_native()
-        f = N.lib().hv_workspace_bytes
-        f.restype = C.c_size_t
-        return int(f(hd, N.i32(n), N.i32(1), N.i32(h), N.i32(w)))
+        return self._workspace_bytes(n, 1, h, w)
 
     def reserve_workspace(self, n, h, w):
         """Grow the native workspace for n latents of h x w (and n images of 8h x 8w) now, e.g. before capturing a CUDA graph."""
@@ -1235,9 +1203,8 @@ class AutoencoderKL(_NativeNet):
         h = self._sync_native()
         xin = self._as_half(x, "image")
         moments = torch.empty((B, 2 * self.config.latent_channels, H // 8, W // 8), device=xin.device, dtype=torch.float16)
-        self._reserve(h, B, 1, H // 8, W // 8)
-        N.check(N.lib().hv_vae_encode(h, N.ptr(xin), N.ptr(moments), N.i32(B), N.i32(H), N.i32(W), None, C.c_size_t(0), N.stream()), h)
-        dist = DiagonalGaussianDistribution(moments.to(x.dtype) if x.dtype != torch.float16 else moments)
+        self._run(N.lib().hv_vae_encode, h, (B, 1, H // 8, W // 8), N.ptr(xin), N.ptr(moments), N.i32(B), N.i32(H), N.i32(W))
+        dist = DiagonalGaussianDistribution(self._from_half(moments, x.dtype))
         if not return_dict:
             return (dist,)
         return AutoencoderKLOutput(latent_dist=dist)
@@ -1254,9 +1221,8 @@ class AutoencoderKL(_NativeNet):
         h = self._sync_native()
         zin = self._as_half(z, "latents")
         out = torch.empty((B, self.config.out_channels, 8 * H, 8 * W), device=zin.device, dtype=torch.float16)
-        self._reserve(h, B, 1, H, W)
-        N.check(N.lib().hv_vae_decode(h, N.ptr(zin), N.ptr(out), N.i32(B), N.i32(H), N.i32(W), None, C.c_size_t(0), N.stream()), h)
-        out = out.to(z.dtype) if z.dtype != torch.float16 else out
+        self._run(N.lib().hv_vae_decode, h, (B, 1, H, W), N.ptr(zin), N.ptr(out), N.i32(B), N.i32(H), N.i32(W))
+        out = self._from_half(out, z.dtype)
         if not return_dict:
             return (out,)
         return DecoderOutput(sample=out)
@@ -1270,29 +1236,7 @@ class AutoencoderKL(_NativeNet):
     def from_pretrained(cls, pretrained_model_path, subfolder=None, torch_dtype=None, **kwargs):
         """diffusers-style loader: ``<path>[/<subfolder>]/config.json`` + ``diffusion_pytorch_model.safetensors`` (or ``.bin``); old
         attention names are converted.  Builds on the CPU; move it with ``.to("cuda", torch.float16)``."""
-        path = os.path.join(str(pretrained_model_path), subfolder) if subfolder is not None else str(pretrained_model_path)
-        with open(os.path.join(path, "config.json")) as f:
-            cfg = {k: v for k, v in json.load(f).items() if not k.startswith("_")}
-        import inspect
-
-        allowed = set(inspect.signature(cls.__init__).parameters) - {"self", "unused"}
-        model = cls(**{k: v for k, v in cfg.items() if k in allowed})
-        st_path = os.path.join(path, "diffusion_pytorch_model.safetensors")
-        if os.path.exists(st_path):
-            from safetensors.torch import load_file
-
-            state = load_file(st_path, device="cpu")
-        else:
-            bin_path = os.path.join(path, "diffusion_pytorch_model.bin")
-            if not os.path.isfile(bin_path):
-                raise FileNotFoundError(f"no weights file found in {path}")
-            state = torch.load(bin_path, map_location="cpu", weights_only=True)
-        missing = model.load_state_dict(state, strict=False).missing_keys
-        if missing:
-            raise RuntimeError(f"{path}: weights missing from the checkpoint: {missing[:5]}{' ...' if len(missing) > 5 else ''}")
-        if torch_dtype is not None:
-            model = model.to(torch_dtype)
-        return model
+        return _from_pretrained(cls, pretrained_model_path, subfolder, require_all=True, torch_dtype=torch_dtype)
 
 
 # --------------------------------------------------------------------------------------------- CLIPVisionModelWithProjection
@@ -1367,8 +1311,6 @@ class CLIPVisionModelWithProjection(_NativeNet):
     supported: quick-GELU MLPs, heads of dimension 64, RGB input.  Inference only.
     """
 
-    _kind = 5
-
     def __init__(
         self,
         hidden_size: int = 768,
@@ -1413,7 +1355,7 @@ class CLIPVisionModelWithProjection(_NativeNet):
     def _hv_config(self):
         c = self.config
         cfg = HvConfig()
-        cfg.kind = 5
+        cfg.kind = N.HV_KIND_CLIP_VISION
         cfg.clip_hidden_size, cfg.clip_layers, cfg.clip_heads = c.hidden_size, c.num_hidden_layers, c.num_attention_heads
         cfg.clip_intermediate_size, cfg.clip_patch_size, cfg.clip_image_size = c.intermediate_size, c.patch_size, c.image_size
         cfg.clip_projection_dim, cfg.clip_layer_norm_eps = c.projection_dim, c.layer_norm_eps
@@ -1425,11 +1367,8 @@ class CLIPVisionModelWithProjection(_NativeNet):
 
     def workspace_bytes(self, batch) -> int:
         """Device workspace of one forward over `batch` images."""
-        hd = self._sync_native()
-        f = N.lib().hv_workspace_bytes
-        f.restype = C.c_size_t
         s = self.config.image_size
-        return int(f(hd, N.i32(batch), N.i32(1), N.i32(s), N.i32(s)))
+        return self._workspace_bytes(batch, 1, s, s)
 
     def reserve_workspace(self, batch):
         """Grow the native workspace for `batch` images now, e.g. before capturing a CUDA graph."""
@@ -1456,10 +1395,9 @@ class CLIPVisionModelWithProjection(_NativeNet):
         pix = self._as_half(pixel_values, "pixel_values")
         embeds = torch.empty((B, c.projection_dim), device=pix.device, dtype=torch.float16)
         hidden = torch.empty((B, (c.image_size // c.patch_size) ** 2 + 1, c.hidden_size), device=pix.device, dtype=torch.float16)
-        self._reserve(h, B, 1, c.image_size, c.image_size)
-        N.check(N.lib().hv_clip_vision_forward(h, N.ptr(pix), N.ptr(embeds), N.ptr(hidden), N.i32(B), None, C.c_size_t(0), N.stream()), h)
-        if self.dtype != torch.float16:
-            embeds, hidden = embeds.to(self.dtype), hidden.to(self.dtype)
+        self._run(N.lib().hv_clip_vision_forward, h, (B, 1, c.image_size, c.image_size), N.ptr(pix), N.ptr(embeds), N.ptr(hidden), N.i32(B))
+        dtype = self.dtype
+        embeds, hidden = self._from_half(embeds, dtype), self._from_half(hidden, dtype)
         if return_dict is False:
             return (embeds, hidden)
         return CLIPVisionModelOutput(image_embeds=embeds, last_hidden_state=hidden)
@@ -1468,26 +1406,5 @@ class CLIPVisionModelWithProjection(_NativeNet):
     def from_pretrained(cls, pretrained_model_path, subfolder=None, torch_dtype=None, **kwargs):
         """transformers-style loader: ``<path>[/<subfolder>]/config.json`` (a ``clip_vision_model`` config) + ``model.safetensors`` (or
         ``pytorch_model.bin``).  Builds on the CPU; move it with ``.to("cuda", torch.float16)``."""
-        path = os.path.join(str(pretrained_model_path), subfolder) if subfolder is not None else str(pretrained_model_path)
-        with open(os.path.join(path, "config.json")) as f:
-            cfg = {k: v for k, v in json.load(f).items() if not k.startswith("_")}
-        import inspect
-
-        allowed = set(inspect.signature(cls.__init__).parameters) - {"self", "unused"}
-        model = cls(**{k: v for k, v in cfg.items() if k in allowed})
-        st_path = os.path.join(path, "model.safetensors")
-        if os.path.exists(st_path):
-            from safetensors.torch import load_file
-
-            state = load_file(st_path, device="cpu")
-        else:
-            bin_path = os.path.join(path, "pytorch_model.bin")
-            if not os.path.isfile(bin_path):
-                raise FileNotFoundError(f"no weights file found in {path}")
-            state = torch.load(bin_path, map_location="cpu", weights_only=True)
-        missing = model.load_state_dict(state, strict=False).missing_keys
-        if missing:
-            raise RuntimeError(f"{path}: weights missing from the checkpoint: {missing[:5]}{' ...' if len(missing) > 5 else ''}")
-        if torch_dtype is not None:
-            model = model.to(torch_dtype)
-        return model
+        return _from_pretrained(cls, pretrained_model_path, subfolder, weights=("model.safetensors", "pytorch_model.bin"), require_all=True,
+                                torch_dtype=torch_dtype)

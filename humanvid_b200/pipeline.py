@@ -166,6 +166,60 @@ class _PipelineBase:
         enc_dtype = next(self.image_encoder.parameters()).dtype if hasattr(self.image_encoder, "parameters") else torch.float16
         return self.image_encoder(pix.to(device, dtype=enc_dtype)).image_embeds
 
+    def _begin(self, ref_image, num_inference_steps, guidance_scale):
+        """(device, CFG on, host timesteps, encoder_hidden_states): the CLIP image embedding as (b, 1, dim), behind a zero unconditional
+        half under CFG."""
+        device = torch.device("cuda") if torch.cuda.is_available() else torch.device("cpu")
+        cfg_on = guidance_scale > 1.0
+        self.scheduler.set_timesteps(num_inference_steps, device=device)
+        timesteps = getattr(self.scheduler, "_host_timesteps", None) or [int(t) for t in self.scheduler.timesteps]
+        ehs = self._clip_embed(ref_image, device).unsqueeze(1)
+        if cfg_on:
+            ehs = torch.cat([torch.zeros_like(ehs), ehs], dim=0)
+        return device, cfg_on, timesteps, ehs
+
+    def _reference_controls(self, cfg_on):
+        """(writer, reader) ReferenceAttentionControls: ``reference_control_cls`` if set, else this package's reader, and its writer around a
+        native reference UNet (no writer otherwise)."""
+        writer_cls, reader_cls = self.reference_control_cls or (None, None)
+        if reader_cls is None:
+            from .modules import ReferenceAttentionControl as reader_cls
+        if writer_cls is None and self.reference_unet is not None:
+            from .modules import ReferenceAttentionControl, UNet2DConditionModel
+            if isinstance(self.reference_unet, UNet2DConditionModel):   # native reference UNet: the native control writes its banks
+                writer_cls = ReferenceAttentionControl
+        writer = writer_cls(self.reference_unet, do_classifier_free_guidance=cfg_on, mode="write", batch_size=1, fusion_blocks="full") \
+            if writer_cls is not None else None
+        reader = reader_cls(self.denoising_unet, do_classifier_free_guidance=cfg_on, mode="read", batch_size=1, fusion_blocks="full")
+        return writer, reader
+
+    def _reference_latents(self, ref_image, height, width, device):
+        vae_dtype = next(self.vae.parameters()).dtype if hasattr(self.vae, "parameters") else torch.float16
+        return self.vae.encode(_to_tensor_image(ref_image, height, width).to(dtype=vae_dtype, device=device)).latent_dist.mean * 0.18215
+
+    def _write_banks(self, writer, reader, ref_latents, ehs, cfg_on, device):
+        """One reference-UNet forward over the reference latents, then hand its banks to the denoising UNet."""
+        if writer is not None:
+            self.reference_unet(ref_latents.repeat((2 if cfg_on else 1), 1, 1, 1), torch.zeros((), dtype=torch.long, device=device),
+                                encoder_hidden_states=ehs, return_dict=False)
+            reader.update(writer)
+
+    @staticmethod
+    def _clear_controls(writer, reader):
+        reader.clear()
+        if writer is not None:
+            writer.clear()
+
+    def _output(self, latents, output_type, return_dict, output_cls):
+        """The latents (output_type "latent") or the decoded frames (a tensor for "tensor", else an ndarray), in `output_cls` when
+        return_dict."""
+        out = latents
+        if output_type != "latent":
+            out = self.decode_latents(latents)
+            if output_type == "tensor":
+                out = torch.from_numpy(out)
+        return output_cls(out) if return_dict else out
+
     def _device_loop_ok(self, eta, callback, context_batch_size, context_queue, latents, cfg_on=True) -> bool:
         """The on-device loop covers what scripts/pose2vid.py uses: native denoising UNet, this package's DDIM scheduler with
         eta = 0, no per-step host callback, one window per UNet call, equally long windows, and CFG on whenever windows overlap.
@@ -226,33 +280,11 @@ class Pose2VideoPipeline(_PipelineBase):
                  num_images_per_prompt=1, eta: float = 0.0, generator=None, output_type: Optional[str] = "tensor", return_dict: bool = True,
                  callback: Optional[Callable] = None, callback_steps: Optional[int] = 1, context_schedule="uniform", context_frames=24,
                  context_stride=1, context_overlap=4, context_batch_size=1, interpolation_factor=1, **kwargs):
-        device = torch.device("cuda") if torch.cuda.is_available() else torch.device("cpu")
-        cfg_on = guidance_scale > 1.0
-        self.scheduler.set_timesteps(num_inference_steps, device=device)
-        timesteps = getattr(self.scheduler, "_host_timesteps", None) or [int(t) for t in self.scheduler.timesteps]
-        batch_size = 1
-
-        clip_image_embeds = self._clip_embed(ref_image, device)
-        encoder_hidden_states = clip_image_embeds.unsqueeze(1)
-        if cfg_on:
-            encoder_hidden_states = torch.cat([torch.zeros_like(encoder_hidden_states), encoder_hidden_states], dim=0)
-
-        writer_cls, reader_cls = self.reference_control_cls or (None, None)
-        if reader_cls is None:
-            from .modules import ReferenceAttentionControl as reader_cls
-        if writer_cls is None and self.reference_unet is not None:
-            from .modules import ReferenceAttentionControl, UNet2DConditionModel
-            if isinstance(self.reference_unet, UNet2DConditionModel):   # native reference UNet: the native control writes its banks
-                writer_cls = ReferenceAttentionControl
-        writer = writer_cls(self.reference_unet, do_classifier_free_guidance=cfg_on, mode="write", batch_size=batch_size, fusion_blocks="full") \
-            if writer_cls is not None else None
-        reader = reader_cls(self.denoising_unet, do_classifier_free_guidance=cfg_on, mode="read", batch_size=batch_size, fusion_blocks="full")
-
-        latents = self.prepare_latents(batch_size * num_images_per_prompt, self.denoising_unet.in_channels, width, height, video_length,
-                                       clip_image_embeds.dtype, device, generator)
-        vae_dtype = next(self.vae.parameters()).dtype if hasattr(self.vae, "parameters") else torch.float16
-        ref_image_tensor = _to_tensor_image(ref_image, height, width).to(dtype=vae_dtype, device=device)
-        ref_image_latents = self.vae.encode(ref_image_tensor).latent_dist.mean * 0.18215
+        device, cfg_on, timesteps, encoder_hidden_states = self._begin(ref_image, num_inference_steps, guidance_scale)
+        writer, reader = self._reference_controls(cfg_on)
+        latents = self.prepare_latents(num_images_per_prompt, self.denoising_unet.in_channels, width, height, video_length, encoder_hidden_states.dtype,
+                                       device, generator)
+        ref_image_latents = self._reference_latents(ref_image, height, width, device)
 
         pose_cond_tensor = torch.cat([_to_tensor_image(p, height, width, (0.0, 1.0)).unsqueeze(2) for p in pose_images], dim=2)
         pose_cond_tensor = pose_cond_tensor.to(device=device, dtype=self.pose_guider.dtype)
@@ -275,19 +307,13 @@ class Pose2VideoPipeline(_PipelineBase):
                 feature_cache[key] = cond
             return cond
 
-        def write_banks():
-            if writer is not None:
-                self.reference_unet(ref_image_latents.repeat((2 if cfg_on else 1), 1, 1, 1), torch.zeros((), dtype=torch.long, device=device),
-                                    encoder_hidden_states=encoder_hidden_states, return_dict=False)
-                reader.update(writer)
-
         # the scheduler is always asked with step = 0 (:495-502): the windows are the same at every timestep
         context_queue = list(context_scheduler(0, num_inference_steps, latents.shape[2], context_frames, context_stride, context_overlap))
         if self._device_loop_ok(eta, callback, context_batch_size, context_queue, latents, cfg_on):
             # ---- SURVEY 8f-2: every per-timestep operation on the device, one CUDA graph per step -------------------------
             from .device_loop import DeviceDenoiseLoop
 
-            write_banks()
+            self._write_banks(writer, reader, ref_image_latents, encoder_hidden_states, cfg_on, device)
             conds = [window_features([c]) for c in context_queue]
             extra = self._loop_kwargs(context_queue, cfg_on)
             loop = self._cached_loop
@@ -314,7 +340,7 @@ class Pose2VideoPipeline(_PipelineBase):
             noise_pred = torch.zeros((latents.shape[0] * (2 if cfg_on else 1), *latents.shape[1:]), device=latents.device, dtype=latents.dtype)
             counter = torch.zeros((1, 1, latents.shape[2], 1, 1), device=latents.device, dtype=latents.dtype)
             if i == 0:
-                write_banks()
+                self._write_banks(writer, reader, ref_image_latents, encoder_hidden_states, cfg_on, device)
             nb = math.ceil(len(context_queue) / context_batch_size)
             global_context = [context_queue[k * context_batch_size : (k + 1) * context_batch_size] for k in range(nb)]
             for context in global_context:
@@ -333,17 +359,10 @@ class Pose2VideoPipeline(_PipelineBase):
             latents = self.scheduler.step(noise_pred, t, latents, eta=eta).prev_sample
             if callback is not None and i % callback_steps == 0:
                 callback(i, t, latents)
-        reader.clear()
-        if writer is not None:
-            writer.clear()
+        self._clear_controls(writer, reader)
         if interpolation_factor > 0:
             latents = self.interpolate_latents(latents, interpolation_factor, device)
-        if output_type == "latent":
-            return latents if not return_dict else Pose2VideoPipelineOutput(videos=latents)
-        images = self.decode_latents(latents)
-        if output_type == "tensor":
-            images = torch.from_numpy(images)
-        return images if not return_dict else Pose2VideoPipelineOutput(videos=images)
+        return self._output(latents, output_type, return_dict, Pose2VideoPipelineOutput)
 
 
 class Pose2ImagePipeline(_PipelineBase):
@@ -353,27 +372,10 @@ class Pose2ImagePipeline(_PipelineBase):
     def __call__(self, ref_image, pose_image, camera_embedding, width, height, num_inference_steps, guidance_scale, num_images_per_prompt=1,
                  eta: float = 0.0, generator=None, output_type: Optional[str] = "tensor", return_dict: bool = True, callback=None,
                  callback_steps: Optional[int] = 1, **kwargs):
-        device = torch.device("cuda") if torch.cuda.is_available() else torch.device("cpu")
-        cfg_on = guidance_scale > 1.0
-        self.scheduler.set_timesteps(num_inference_steps, device=device)
-        timesteps = getattr(self.scheduler, "_host_timesteps", None) or [int(t) for t in self.scheduler.timesteps]
-        clip_image_embeds = self._clip_embed(ref_image, device)
-        ehs = clip_image_embeds.unsqueeze(1)
-        if cfg_on:
-            ehs = torch.cat([torch.zeros_like(ehs), ehs], dim=0)
-        writer_cls, reader_cls = self.reference_control_cls or (None, None)
-        if reader_cls is None:
-            from .modules import ReferenceAttentionControl as reader_cls
-        if writer_cls is None and self.reference_unet is not None:
-            from .modules import ReferenceAttentionControl, UNet2DConditionModel
-            if isinstance(self.reference_unet, UNet2DConditionModel):   # native reference UNet: the native control writes its banks
-                writer_cls = ReferenceAttentionControl
-        writer = writer_cls(self.reference_unet, do_classifier_free_guidance=cfg_on, mode="write", batch_size=1, fusion_blocks="full") \
-            if writer_cls is not None else None
-        reader = reader_cls(self.denoising_unet, do_classifier_free_guidance=cfg_on, mode="read", batch_size=1, fusion_blocks="full")
-        latents = self.prepare_latents(num_images_per_prompt, self.denoising_unet.in_channels, width, height, 1, clip_image_embeds.dtype, device, generator)
-        vae_dtype = next(self.vae.parameters()).dtype if hasattr(self.vae, "parameters") else torch.float16
-        ref_latents = self.vae.encode(_to_tensor_image(ref_image, height, width).to(dtype=vae_dtype, device=device)).latent_dist.mean * 0.18215
+        device, cfg_on, timesteps, ehs = self._begin(ref_image, num_inference_steps, guidance_scale)
+        writer, reader = self._reference_controls(cfg_on)
+        latents = self.prepare_latents(num_images_per_prompt, self.denoising_unet.in_channels, width, height, 1, ehs.dtype, device, generator)
+        ref_latents = self._reference_latents(ref_image, height, width, device)
         pose = _to_tensor_image(pose_image, height, width, (0.0, 1.0)).unsqueeze(2).to(device=device, dtype=self.pose_guider.dtype)
         pose_fea = self.pose_guider(pose)
         camera_embedding = camera_embedding.to(device=device, dtype=self.camera_pose_encoder.dtype)
@@ -388,10 +390,8 @@ class Pose2ImagePipeline(_PipelineBase):
             cond = cond.repeat(latents.shape[0] // cond.shape[0], 1, 1, 1, 1)
         cond = cond.repeat(2 if cfg_on else 1, 1, 1, 1, 1)
         for i, t in enumerate(timesteps):
-            if i == 0 and writer is not None:
-                self.reference_unet(ref_latents.repeat((2 if cfg_on else 1), 1, 1, 1), torch.zeros((), dtype=torch.long, device=device),
-                                    encoder_hidden_states=ehs, return_dict=False)
-                reader.update(writer)
+            if i == 0:
+                self._write_banks(writer, reader, ref_latents, ehs, cfg_on, device)
             x = self.scheduler.scale_model_input(latents.repeat(2 if cfg_on else 1, 1, 1, 1, 1), t)
             noise_pred = self.denoising_unet(x, t, encoder_hidden_states=ehs, pose_cond_fea=cond, return_dict=False)[0]
             if cfg_on:
@@ -400,12 +400,5 @@ class Pose2ImagePipeline(_PipelineBase):
             latents = self.scheduler.step(noise_pred, t, latents, eta=eta).prev_sample
             if callback is not None and i % callback_steps == 0:
                 callback(i, t, latents)
-        reader.clear()
-        if writer is not None:
-            writer.clear()
-        if output_type == "latent":
-            return latents if not return_dict else Pose2ImagePipelineOutput(images=latents)
-        image = self.decode_latents(latents)
-        if output_type == "tensor":
-            image = torch.from_numpy(image)
-        return image if not return_dict else Pose2ImagePipelineOutput(images=image)
+        self._clear_controls(writer, reader)
+        return self._output(latents, output_type, return_dict, Pose2ImagePipelineOutput)

@@ -207,6 +207,31 @@ def test_from_pretrained_2d_loading_flow(tmp_path):
         UNet3DConditionModel.from_pretrained_2d(tmp_path / "nowhere", mm_file, unet_additional_kwargs=extra)
 
 
+def test_reference_unet2d_from_pretrained(tmp_path):
+    """The writer UNet's diffusers-style loader: config.json keys its __init__ does not take are dropped, SD checkpoint keys it has no
+    parameter for (conv_norm_out / conv_out) are ignored, and a directory without a weights file raises FileNotFoundError."""
+    import json
+
+    from safetensors.torch import save_file
+
+    from humanvid_b200 import UNet2DConditionModel
+
+    src = O.synthetic_init(O.UNet2DConditionModel(block_out_channels=(32, 64, 128, 128), cross_attention_dim=64), seed=5)
+    sd = {k: v.clone().contiguous() for k, v in src.state_dict().items()}
+    d = tmp_path / "unet"
+    d.mkdir()
+    cfg = {"_class_name": "UNet2DConditionModel", "block_out_channels": [32, 64, 128, 128], "cross_attention_dim": 64, "sample_size": 64,
+           "some_future_key": 1}
+    json.dump(cfg, open(d / "config.json", "w"))
+    with pytest.raises(FileNotFoundError):
+        UNet2DConditionModel.from_pretrained(tmp_path, subfolder="unet")
+    save_file({**sd, "conv_out.weight": torch.zeros(4, 32, 3, 3), "conv_out.bias": torch.zeros(4)}, str(d / "diffusion_pytorch_model.safetensors"))
+    m = UNet2DConditionModel.from_pretrained(tmp_path, subfolder="unet")
+    got = m.state_dict()
+    assert set(got) == set(sd) and all(torch.equal(got[k], sd[k]) for k in sd)
+    assert m.config.sample_size == 64 and m.config.block_out_channels == [32, 64, 128, 128]
+
+
 def test_native_fingerprint_tracks_parameter_edits():
     """_NativeNet._versions() decides on every forward whether the packed device weights are stale.  Its tensor list is cached per epoch
     (3 ms of module-tree walking per forward otherwise); the fingerprint must still move on an in-place edit of ANY parameter or buffer, on
