@@ -776,6 +776,10 @@ class UNet2DConditionModel(_NativeNet):
     def _hv_config(self):
         return _sd15_hv_config(self.config, N.HV_KIND_UNET2D_REF)
 
+    # debug taps: the denoising UNet's, at one frame (debug_tap_plan(B, 1, h, w))
+    debug_tap_plan = UNet3DConditionModel.debug_tap_plan
+    debug_set_taps = UNet3DConditionModel.debug_set_taps
+
     @torch.no_grad()
     def forward(self, sample: torch.Tensor, timestep: Union[torch.Tensor, float, int], encoder_hidden_states: torch.Tensor,
                 class_labels: Optional[torch.Tensor] = None, timestep_cond=None, attention_mask=None, cross_attention_kwargs=None,

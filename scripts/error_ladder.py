@@ -20,6 +20,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import humanvid_b200 as hv  # noqa: E402
 from oracle import hv_oracle as O  # noqa: E402
+from oracle.block_replay import replay_blocks, to_nhwc  # noqa: E402
 
 MM_KW = dict(num_attention_heads=8, num_transformer_block=1, attention_block_types=["Temporal_Self", "Temporal_Self"],
              temporal_position_encoding=True, temporal_position_encoding_max_len=32, temporal_attention_dim_div=1)
@@ -28,11 +29,6 @@ MM_KW = dict(num_attention_heads=8, num_transformer_block=1, attention_block_typ
 def rel(a, b):
     a, b = a.float(), b.float()
     return float((a - b).norm() / (b.norm() + 1e-20))
-
-
-def to_nhwc(t):  # (B, C, F, H, W) -> (B*F, H, W, C)
-    b, c, f, h, w = t.shape
-    return t.permute(0, 2, 3, 4, 1).reshape(b * f, h, w, c)
 
 
 def run_oracle(ora, names, x, t, ehs, pose, visit):
@@ -110,51 +106,11 @@ def main():
 
     # ---- isolated per-block error: the oracle's block in fp32 applied to the NATIVE block's own input (the native taps of its
     # predecessors), against the native block's output -- "identical inputs, per tensor" (north_star), free of the error the input
-    # already carried.  (Reference banks change the attention inputs, so this column is produced for the bank-free run only.)
+    # already carried.  The banks set above are the oracle's fp32 banks, so the replay reads them as the whole forward did.
     iso = {}
-    if not a.banks:
-        B = 2
-
-        def to_ncfhw(t):  # (B*F, H, W, C) fp16 -> (B, C, F, H, W) fp32
-            nf, hh, ww, c = t.shape
-            return t.reshape(B, nf // B, hh, ww, c).permute(0, 4, 1, 2, 3).float().contiguous()
-
-        mods = dict(ora.named_modules())
-        with torch.no_grad():
-            tt = torch.tensor([a.timestep], device=dev).expand(B)
-            emb = ora.time_embedding(O.timestep_sincos(tt, ora.conv_in.out_channels).float())
-            ehs32 = ehs.float()
-            iso["conv_in"] = rel(native["conv_in"], to_nhwc(ora.conv_in(x.float()) + pose.float()))
-            # the skip stack of the forward (unet_3d.py:486-506): conv_in, then every down layer's last module, then the block's downsampler
-            skips = ["conv_in"]
-            for n in names:
-                if n.startswith("down_blocks"):
-                    blk, kind, idx = n.rsplit(".", 2)
-                    if kind == "downsamplers":
-                        skips.append(n)
-                    elif kind == "resnets":
-                        skips.append(n)                      # provisional: replaced by the layer's later modules below
-                    else:
-                        skips[-1] = n                        # attentions.j / motion_modules.j follow resnets.j of the same layer
-            prev = "conv_in"
-            for n in names[1:]:
-                h_in = to_ncfhw(native[prev])
-                kind = n.split(".")[-2]
-                if n.startswith("up_blocks") and kind == "resnets":
-                    h_in = torch.cat([h_in, to_ncfhw(native[skips.pop()])], dim=1)
-                m = mods[n]
-                if kind == "resnets":
-                    out = m(h_in, emb)
-                elif kind == "attentions":
-                    out = m(h_in, ehs32)
-                elif kind == "upsamplers":
-                    out = m(h_in, None)
-                else:   # motion_modules, downsamplers
-                    out = m(h_in)
-                iso[n] = rel(native[n], to_nhwc(out))
-                del out, h_in
-                prev = n
-            assert not skips, skips
+    for n, out in replay_blocks(ora, names, native, x, a.timestep, ehs, pose):
+        iso[n] = rel(native[n], out)
+        del out
 
     os.makedirs(os.path.dirname(a.out) or ".", exist_ok=True)
     with open(a.out, "w") as f:

@@ -60,16 +60,33 @@ def half_step(v, s):
 
 def _ff_emulated(ff, x):
     """oracle FeedForward (GEGLU proj -> Linear) with e4m3 quantise-dequantise at the FP8 path's points: the LayerNorm output per token,
-    the weights per row, the GEGLU output per (token, 128 columns)."""
+    the weights per row, the GEGLU output per (token, 128 columns).  The scales and e4m3 values are formed in fp32 as the kernels form them;
+    the arithmetic between the quantisation points runs in x's dtype (fp32, or fp64 for a reference of the emulation)."""
     proj, lin2 = ff.net[0].proj, ff.net[2]
-    h = torch.nn.functional.linear(qdq(x), qdq(proj.weight), proj.bias)
+    h = torch.nn.functional.linear(qdq(x).to(x.dtype), qdq(proj.weight).to(x.dtype), proj.bias)
     hidden, gate = h.chunk(2, dim=-1)
-    y = qdq(hidden * torch.nn.functional.gelu(gate), 128)
-    return torch.nn.functional.linear(y, qdq(lin2.weight), lin2.bias)
+    y = qdq(hidden * torch.nn.functional.gelu(gate), 128).to(x.dtype)
+    return torch.nn.functional.linear(y, qdq(lin2.weight).to(x.dtype), lin2.bias)
+
+
+def ff_flip_bound(ff, x):
+    """Per output element of the emulated FeedForward on x, the most that flipped e4m3 roundings of its GEGLU output can move it.
+
+    The native FP8 path quantises a GEGLU output that carries the fp16 path's error; where that error carries a value across an e4m3
+    rounding midpoint, the value lands one e4m3 spacing (two half_steps) from the emulation's.  Through ff2 this moves output i by at most
+    sum_j |W2[i, j]| 2 half_step(y_j): the bound for every value of the row flipping at once."""
+    proj, lin2 = ff.net[0].proj, ff.net[2]
+    h = torch.nn.functional.linear(qdq(x).to(x.dtype), qdq(proj.weight).to(x.dtype), proj.bias)
+    hidden, gate = h.chunk(2, dim=-1)
+    v = hidden * torch.nn.functional.gelu(gate)
+    q, s = quantize(v, 128)
+    y = dequantize(q, s, 128)
+    step = 2 * half_step(y, s.repeat_interleave(128, dim=-1)[..., : v.shape[-1]])
+    return torch.nn.functional.linear(step.to(x.dtype), qdq(lin2.weight).to(x.dtype).abs())
 
 
 class emulate_fp8_linears:
-    """Context manager: the fp32 oracle UNet with the FP8 mode's quantisation inserted in the feed-forwards FP8 mode runs on e4m3 (those
+    """Context manager: the oracle UNet (fp32, or fp64) with the FP8 mode's quantisation inserted in the feed-forwards FP8 mode runs on e4m3 (those
     of width >= min_dim; the LayerNorm in front of each is the caller of FeedForward, so quantising its input is quantising the LayerNorm's
     output)."""
 

@@ -1,6 +1,6 @@
-"""Per-block parity with identical inputs (north_star: "<= 1e-3 rel fp16 per tensor"): scripts/error_ladder.py feeds every block of the
-oracle (fp32) with the NATIVE block's own input and compares outputs -- the error each block adds by itself, free of what its input already
-carried.  Run here on the narrow UNet (max isolated per-block error 3.1e-4 on an H100 SXM at 700 W; scripts/error_ladder.py runs the full size)."""
+"""Accumulated drift through the network (scripts/error_ladder.py on the narrow UNet): at every block, native stays no further from the fp32
+oracle than the reference's own fp16 path.  The isolated per-block error -- every block on its own input -- is asserted per frame, row and
+element against fp64 by tests/test_block_parity_gpu.py, at this shape among others; here it is only reported."""
 import os
 import re
 import subprocess
@@ -14,7 +14,7 @@ pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def test_every_block_is_within_1e3_of_fp32_on_its_own_input(tmp_path):
+def test_native_drift_never_exceeds_fp16_eager(tmp_path):
     out = str(tmp_path / "ladder.txt")
     p = subprocess.run([sys.executable, os.path.join(ROOT, "scripts", "error_ladder.py"), "--narrow", "--hw", "32", "32", "--frames", "6", "--out", out],
                        capture_output=True, text=True, timeout=900, cwd=ROOT)
@@ -24,7 +24,6 @@ def test_every_block_is_within_1e3_of_fp32_on_its_own_input(tmp_path):
     rows = [l.split() for l in txt.splitlines() if l and not l.startswith("#")]
     nat, eag = [float(r[-4]) for r in rows], [float(r[-3]) for r in rows]
     report(f"error ladder (narrow UNet, 66 taps): max isolated per-block error {iso:.2e}; accumulated native/fp32 max {max(nat):.2e} vs fp16-eager/fp32 max {max(eag):.2e}")
-    assert iso <= 1e-3                       # measured ~3e-4: one fp16 rounding of the block's output
     assert len(rows) >= 60
     # accumulated through the network, native never drifts further from fp32 than the reference's own fp16 path does (5 % slack per tap)
     assert all(n <= 1.05 * e + 1e-5 for n, e in zip(nat, eag)), [(r[0], n, e) for r, n, e in zip(rows, nat, eag) if n > 1.05 * e + 1e-5][:5]
