@@ -44,14 +44,31 @@ constexpr int kMathWarps = 8;       // every math warp releases a ring slot once
 // 65536 registers over 384 threads: the producer keeps 40, the two math warpgroups get 232 each (128 accumulators at N = 256)
 constexpr uint32_t kProducerRegs = 40, kMathRegs = 232;
 
-// Shared memory: [B panel (BST)] [ring: stages x (A tile [+ B tile])] [epilogue staging: epi_slabs x SLAB_BYTES] [barriers]
-template <int BLOCK_N>
-struct Cfg {
-  static constexpr int kBTileBytes = BLOCK_N * BLOCK_K * 2;
-  static constexpr int kStageBytes = A_TILE_BYTES + kBTileBytes;
-  static constexpr int kBarBytes = (2 * kMaxStages + 3) * 8;   // full[8] empty[8] bpanel epi_ready epi_staged
-  static constexpr int kFixed = kBarBytes + 1024;              // + alignment slack
+// Shared memory, from the 1024-byte aligned base: [B panel (BST): num_k_blocks B tiles] [ring: stages x (A tile [+ B tile])]
+// [epilogue staging: slabs x SLAB_BYTES] [barriers: full[8] empty[8] bpanel epi_ready epi_staged].
+struct SmemLayout {
+  int b_tile, stage;  // bytes of one B tile and of one ring stage
+  int bytes;          // the dynamic allocation, with the alignment slack
 };
+__host__ __device__ constexpr SmemLayout smem_layout(int block_n, bool bst, int num_k_blocks, int stages, int slabs) {
+  SmemLayout l{};
+  l.b_tile = block_n * BLOCK_K * 2;
+  l.stage = A_TILE_BYTES + (bst ? 0 : l.b_tile);
+  l.bytes = (bst ? num_k_blocks * l.b_tile : 0) + stages * l.stage + slabs * SLAB_BYTES + (2 * kMaxStages + 3) * 8 + 1024;
+  return l;
+}
+
+// M tiles (conv: boxes, times the four output parities of the up-convolution) and N tiles (batched B: per item) of a problem.
+struct TileCounts {
+  int m, n, n_per_batch;
+};
+__host__ __device__ __forceinline__ TileCounts tile_counts(const GemmProblem& p, int block_n) {
+  TileCounts t;
+  t.m = p.a_mode == A_LINEAR ? (p.M + BLOCK_M - 1) / BLOCK_M : p.tiles_n * p.tiles_y * p.tiles_x * (p.a_mode == A_UPCONV2X2 ? 4 : 1);
+  t.n_per_batch = p.b_batch ? (p.b_rows + block_n - 1) / block_n : 0;
+  t.n = p.b_batch ? p.b_batch * t.n_per_batch : (p.N + block_n - 1) / block_n;
+  return t;
+}
 
 // First output column of tile n_blk and the number of its 32-column slabs that hold written columns (< n_valid).
 template <int BLOCK_N>
@@ -102,15 +119,15 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ CUtensorMap map_a1,
             const __grid_constant__ CUtensorMap map_b, const __grid_constant__ CUtensorMap map_out,
             const __grid_constant__ CUtensorMap map_res, const GemmProblem p, const GemmEpilogue e) {
-  using C = Cfg<BLOCK_N>;
   constexpr int KB = FP8 ? 2 * BLOCK_K : BLOCK_K;   // elements per k-block
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int nstages = p.stages;
   const int nslab = p.epi_slabs;
-  constexpr int kRingStageBytes = BST ? A_TILE_BYTES : C::kStageBytes;
-  uint8_t* ring = smem + (BST ? p.num_k_blocks * C::kBTileBytes : 0);
-  uint8_t* stg = ring + nstages * kRingStageBytes;
+  // smem_layout's regions, chained pointer by pointer: offsets from the base changed the SASS of every instantiation
+  constexpr SmemLayout kL = smem_layout(BLOCK_N, BST, 0, 0, 0);
+  uint8_t* ring = smem + (BST ? p.num_k_blocks * kL.b_tile : 0);
+  uint8_t* stg = ring + nstages * kL.stage;
   uint64_t* bar_full = reinterpret_cast<uint64_t*>(stg + nslab * SLAB_BYTES);
   uint64_t* bar_empty = bar_full + kMaxStages;
   uint64_t* bar_bpanel = bar_empty + kMaxStages;
@@ -120,10 +137,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  const int m_tiles = p.a_mode == A_LINEAR ? (p.M + BLOCK_M - 1) / BLOCK_M : p.tiles_n * p.tiles_y * p.tiles_x * (p.a_mode == A_UPCONV2X2 ? 4 : 1);
-  const int n_per_batch = p.b_batch ? (p.b_rows + BLOCK_N - 1) / BLOCK_N : 0;
-  const int n_tiles = p.b_batch ? p.b_batch * n_per_batch : (p.N + BLOCK_N - 1) / BLOCK_N;
-  const int num_tiles = m_tiles * n_tiles;
+  const TileCounts tiles = tile_counts(p, BLOCK_N);
+  const int n_tiles = tiles.n, n_per_batch = tiles.n_per_batch, num_tiles = tiles.m * tiles.n;
   const int nkb = p.num_k_blocks;
 
   if (threadIdx.x == 0) {
@@ -152,18 +167,18 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ 
       int stage = 0;
       uint32_t phase = 0;
       if (BST && static_cast<int>(blockIdx.x) < num_tiles) {
-        mbar_arrive_expect_tx(bar_bpanel, nkb * C::kBTileBytes);
+        mbar_arrive_expect_tx(bar_bpanel, nkb * kL.b_tile);
         for (int kb = 0; kb < nkb; ++kb)
-          tma_load_2d(smem + kb * C::kBTileBytes, &map_b, bar_bpanel, kb * KB, (blockIdx.x % n_tiles) * BLOCK_N);
+          tma_load_2d(smem + kb * kL.b_tile, &map_b, bar_bpanel, kb * KB, (blockIdx.x % n_tiles) * BLOCK_N);
       }
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int m_blk = tile / n_tiles, n_blk = tile % n_tiles;
         const TileCoord tc = tile_coord(p, m_blk);
         for (int kb = 0; kb < nkb; ++kb) {
           mbar_wait(&bar_empty[stage], phase ^ 1);
-          uint8_t* sa = ring + stage * kRingStageBytes;
+          uint8_t* sa = ring + stage * kL.stage;
           uint8_t* sb = sa + A_TILE_BYTES;
-          mbar_arrive_expect_tx(&bar_full[stage], kRingStageBytes);
+          mbar_arrive_expect_tx(&bar_full[stage], kL.stage);
           if (p.a_mode == A_LINEAR) {
             if (p.k_split == 0 || kb < p.k_split)
               tma_load_2d(sa, &map_a0, &bar_full[stage], kb * KB, tc.m0);
@@ -274,9 +289,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ 
     int prev_stage = -1;
     for (int kb = 0; kb < nkb; ++kb) {
       mbar_wait(&bar_full[stage], phase);
-      const uint32_t sa = smem_u32(ring + stage * kRingStageBytes);
+      const uint32_t sa = smem_u32(ring + stage * kL.stage);
       const uint64_t adesc = gmma_desc_k_sw128(sa + wg * (A_TILE_BYTES / 2));
-      const uint64_t bdesc = gmma_desc_k_sw128(BST ? smem_u32(smem + kb * C::kBTileBytes) : sa + A_TILE_BYTES);
+      const uint64_t bdesc = gmma_desc_k_sw128(BST ? smem_u32(smem + kb * kL.b_tile) : sa + A_TILE_BYTES);
+      // the unpromoted FP8 k-block repeats the fp16 one: a shared helper changed the SASS of the 256-wide FP8 instantiations
       if constexpr (FP8) {
         bool promoted = false;
         if constexpr (kPromote) {
@@ -335,7 +351,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ 
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
         rt[hh] = wg * 64 + wq * 16 + (lane >> 2) + 8 * hh;
-        long long row;
+        long long row;   // the register path's mapping without up-conv parities: one shared helper changed the fp16 SASS
         if (p.a_mode == A_LINEAR) {
           row = tc.m0 + rt[hh];
           ok[hh] = row < p.M;
@@ -443,6 +459,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ 
         for (int j = 0; j < BLOCK_N / 8; ++j) {
           const int col = tile_col0 + 8 * j + 2 * quad;
           if (col < col_lim) {
+            // the staged path's chain again: as one inlined helper it made every fp16 instantiation ~25 % longer
             float v0 = acc[4 * j + 2 * hh] + rowbias, v1 = acc[4 * j + 2 * hh + 1] + rowbias;
             if constexpr (FP8) {
               const float2 sw = __ldg(reinterpret_cast<const float2*>(e.w_scale + col));
@@ -477,18 +494,25 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ 
             *reinterpret_cast<uint32_t*>(out + col) = pack_h2(v0, v1);
           }
         }
-      } else if constexpr (FP8) {
-        // GEGLU on dequantised accumulators; with out8 the 128 outputs of the row are quantised to e4m3 with one scale, their amax
+      } else {
+        // GEGLU (BLOCK_N == 256): tile columns [0,128) are "hidden", [128,256) the matching "gate" rows of the packed weight.  FP8:
+        // on dequantised accumulators; with out8 the 128 outputs of the row are quantised to e4m3 with one scale, their amax
         // reduced over the quad of lanes that hold the row (the geglu value replaces the hidden accumulator it came from)
-        float amax = 0.f;
+        [[maybe_unused]] float amax = 0.f;
 #pragma unroll
         for (int j = 0; j < BLOCK_N / 16; ++j) {
           const int hcol = n_blk * BLOCK_N + 8 * j + 2 * quad;
           const int ocol = n_blk * (BLOCK_N / 2) + 8 * j + 2 * quad;
-          const float2 swh = __ldg(reinterpret_cast<const float2*>(e.w_scale + hcol));
-          const float2 swg = __ldg(reinterpret_cast<const float2*>(e.w_scale + hcol + BLOCK_N / 2));
-          float h0 = acc[4 * j + 2 * hh] * rs * swh.x, h1 = acc[4 * j + 2 * hh + 1] * rs * swh.y;
-          float g0 = acc[4 * (j + BLOCK_N / 16) + 2 * hh] * rs * swg.x, g1 = acc[4 * (j + BLOCK_N / 16) + 2 * hh + 1] * rs * swg.y;
+          float h0 = acc[4 * j + 2 * hh], h1 = acc[4 * j + 2 * hh + 1];
+          float g0 = acc[4 * (j + BLOCK_N / 16) + 2 * hh], g1 = acc[4 * (j + BLOCK_N / 16) + 2 * hh + 1];
+          if constexpr (FP8) {
+            const float2 swh = __ldg(reinterpret_cast<const float2*>(e.w_scale + hcol));
+            const float2 swg = __ldg(reinterpret_cast<const float2*>(e.w_scale + hcol + BLOCK_N / 2));
+            h0 = h0 * rs * swh.x;
+            h1 = h1 * rs * swh.y;
+            g0 = g0 * rs * swg.x;
+            g1 = g1 * rs * swg.y;
+          }
           if (has_bias) {
             const float2 bh = ldh2(e.bias + hcol), bg = ldh2(e.bias + hcol + BLOCK_N / 2);
             h0 += bh.x;
@@ -496,16 +520,20 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ 
             g0 += bg.x;
             g1 += bg.y;
           }
-          const float o0 = geglu1(h0, g0), o1 = geglu1(h1, g1);
-          if (e.out8 != nullptr) {
-            acc[4 * j + 2 * hh] = o0;
-            acc[4 * j + 2 * hh + 1] = o1;
-            amax = fmaxf(amax, fmaxf(fabsf(o0), fabsf(o1)));
+          if constexpr (FP8) {
+            const float o0 = geglu1(h0, g0), o1 = geglu1(h1, g1);
+            if (e.out8 != nullptr) {
+              acc[4 * j + 2 * hh] = o0;
+              acc[4 * j + 2 * hh + 1] = o1;
+              amax = fmaxf(amax, fmaxf(fabsf(o0), fabsf(o1)));
+            } else if (ocol < e.n_valid) {
+              *reinterpret_cast<uint32_t*>(out + ocol) = pack_h2(o0, o1);
+            }
           } else if (ocol < e.n_valid) {
-            *reinterpret_cast<uint32_t*>(out + ocol) = pack_h2(o0, o1);
+            *reinterpret_cast<uint32_t*>(out + ocol) = pack_h2(geglu1(h0, g0), geglu1(h1, g1));
           }
         }
-        if (e.out8 != nullptr) {
+        if (FP8 && e.out8 != nullptr) {
           const unsigned qmask = 0xFu << (lane & 28);
           amax = fmaxf(amax, __shfl_xor_sync(qmask, amax, 1));
           amax = fmaxf(amax, __shfl_xor_sync(qmask, amax, 2));
@@ -515,23 +543,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ 
           for (int j = 0; j < BLOCK_N / 16; ++j)
             *reinterpret_cast<uint16_t*>(o8 + 8 * j + 2 * quad) = e4m3x2(acc[4 * j + 2 * hh], acc[4 * j + 2 * hh + 1], inv);
           if (quad == 0) e.out8_scale[row * e.out8_scale_ld + n_blk] = e4m3_scale(amax);
-        }
-      } else {
-        // GEGLU (BLOCK_N == 256): tile columns [0,128) are "hidden", [128,256) the matching "gate" rows of the packed weight
-#pragma unroll
-        for (int j = 0; j < BLOCK_N / 16; ++j) {
-          const int hcol = n_blk * BLOCK_N + 8 * j + 2 * quad;
-          const int ocol = n_blk * (BLOCK_N / 2) + 8 * j + 2 * quad;
-          float h0 = acc[4 * j + 2 * hh], h1 = acc[4 * j + 2 * hh + 1];
-          float g0 = acc[4 * (j + BLOCK_N / 16) + 2 * hh], g1 = acc[4 * (j + BLOCK_N / 16) + 2 * hh + 1];
-          if (has_bias) {
-            const float2 bh = ldh2(e.bias + hcol), bg = ldh2(e.bias + hcol + BLOCK_N / 2);
-            h0 += bh.x;
-            h1 += bh.y;
-            g0 += bg.x;
-            g1 += bg.y;
-          }
-          if (ocol < e.n_valid) *reinterpret_cast<uint32_t*>(out + ocol) = pack_h2(geglu1(h0, g0), geglu1(h1, g1));
         }
       }
     }
@@ -568,19 +579,18 @@ void choose_conv_box(int NF, int H, int W, int* bn, int* bh, int* bw) {
 // three A stages must fit beside at least one slab, and every CTA must get at least two tiles of its n_blk; slabs come before
 // A stages beyond three.
 static bool plan_smem(int block_n, bool bst, int slabs_wanted, int num_k_blocks, int* stages, int* slabs) {
-  const int fixed = (2 * kMaxStages + 3) * 8 + 1024;
-  const int btile = block_n * BLOCK_K * 2;
   if (!bst) {
+    const SmemLayout l = smem_layout(block_n, false, num_k_blocks, 0, slabs_wanted);
     *slabs = slabs_wanted;
-    *stages = (kMaxSmem - fixed - slabs_wanted * SLAB_BYTES) / (A_TILE_BYTES + btile);
+    *stages = (kMaxSmem - l.bytes) / l.stage;
     if (*stages > kMaxRingStages) *stages = kMaxRingStages;
     return *stages >= 2;
   }
-  const int avail = kMaxSmem - fixed - num_k_blocks * btile;
-  int sl = (avail - 3 * A_TILE_BYTES) / SLAB_BYTES;
+  const int stage = smem_layout(block_n, true, num_k_blocks, 0, 0).stage;
+  int sl = (kMaxSmem - smem_layout(block_n, true, num_k_blocks, 3, 0).bytes) / SLAB_BYTES;
   if (sl > slabs_wanted) sl = slabs_wanted;
   if (sl < (slabs_wanted ? 1 : 0)) return false;
-  int st = (avail - sl * SLAB_BYTES) / A_TILE_BYTES;
+  int st = (kMaxSmem - smem_layout(block_n, true, num_k_blocks, 0, sl).bytes) / stage;
   if (st > kMaxStages) st = kMaxStages;
   if (st < 3) return false;
   *stages = st;
@@ -588,15 +598,9 @@ static bool plan_smem(int block_n, bool bst, int slabs_wanted, int num_k_blocks,
   return true;
 }
 
-static int smem_bytes(int block_n, bool bst, int num_k_blocks, int stages, int slabs) {
-  const int btile = block_n * BLOCK_K * 2;
-  return (bst ? num_k_blocks * btile : 0) + stages * (A_TILE_BYTES + (bst ? 0 : btile)) + slabs * SLAB_BYTES + (2 * kMaxStages + 3) * 8 + 1024;
-}
-
 template <int BN, bool BST, bool FP8>
 static cudaError_t launch_t(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const CUtensorMap& out, const CUtensorMap& res,
                             GemmProblem p, const GemmEpilogue& e, const GemmPlan& plan, cudaStream_t stream) {
-  static_assert(Cfg<BN>::kFixed == (2 * kMaxStages + 3) * 8 + 1024, "plan_smem and the kernel lay out the barriers alike");
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t err = cudaFuncSetAttribute(gemm_kernel<BN, BST, FP8>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
@@ -605,16 +609,29 @@ static cudaError_t launch_t(const CUtensorMap& a0, const CUtensorMap& a1, const 
   }
   p.stages = plan.stages;
   p.epi_slabs = plan.epi_slabs;
-  const int smem = smem_bytes(BN, BST, p.num_k_blocks, plan.stages, plan.epi_slabs);
+  const int smem = smem_layout(BN, BST, p.num_k_blocks, plan.stages, plan.epi_slabs).bytes;
   gemm_kernel<BN, BST, FP8><<<plan.grid, GEMM_THREADS, smem, stream>>>(a0, a1, b, out, res, p, e);
   return cudaGetLastError();
 }
 
+// The <BLOCK_N, BST> instantiation of the fp16 or the e4m3 kernel that runs (block_n, plan).
+template <bool FP8>
+static cudaError_t launch_any(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const CUtensorMap& out, const CUtensorMap& res,
+                              const GemmProblem& p, const GemmEpilogue& e, int block_n, const GemmPlan& plan, cudaStream_t stream) {
+  if (plan.bst_stages > 0) {
+    if (block_n == 256) return launch_t<256, true, FP8>(a0, a1, b, out, res, p, e, plan, stream);
+    if (block_n == 160) return launch_t<160, true, FP8>(a0, a1, b, out, res, p, e, plan, stream);
+    return launch_t<128, true, FP8>(a0, a1, b, out, res, p, e, plan, stream);
+  }
+  if (block_n == 256) return launch_t<256, false, FP8>(a0, a1, b, out, res, p, e, plan, stream);
+  if (block_n == 160) return launch_t<160, false, FP8>(a0, a1, b, out, res, p, e, plan, stream);
+  return launch_t<128, false, FP8>(a0, a1, b, out, res, p, e, plan, stream);
+}
+
 bool plan_gemm(const GemmProblem& p, int block_n, int num_sms, GemmPlan* plan) {
   if (block_n != 128 && block_n != 160 && block_n != 256) return false;
-  const int m_tiles = p.a_mode == A_LINEAR ? (p.M + BLOCK_M - 1) / BLOCK_M : p.tiles_n * p.tiles_y * p.tiles_x * (p.a_mode == A_UPCONV2X2 ? 4 : 1);
-  const int n_tiles = p.b_batch ? p.b_batch * ((p.b_rows + block_n - 1) / block_n) : (p.N + block_n - 1) / block_n;
-  const int tiles = m_tiles * n_tiles;
+  const TileCounts t = tile_counts(p, block_n);
+  const int tiles = t.m * t.n;
   if (tiles <= 0 || p.num_k_blocks <= 0) return false;
   // Staged epilogue for tiles up to 160 wide on outputs up to 640 columns (the level-0/1 linears and the 3x3 convolutions up to 640
   // channels: up to 28 % faster per launch on an H100 SXM at 700 W, most of all with a residual).  Kept on register stores, where
@@ -626,13 +643,13 @@ bool plan_gemm(const GemmProblem& p, int block_n, int num_sms, GemmPlan* plan) {
   plan->bst_stages = 0;
   plan->grid = tiles < num_sms ? tiles : num_sms;
   if (!plan_smem(block_n, false, slabs, p.num_k_blocks, &plan->stages, &plan->epi_slabs)) return false;
-  if (p.a_mode == A_LINEAR && !p.b_batch && n_tiles <= num_sms) {
-    const int per_col = num_sms / n_tiles;  // CTAs sharing one n_blk
+  if (p.a_mode == A_LINEAR && !p.b_batch && t.n <= num_sms) {
+    const int per_col = num_sms / t.n;  // CTAs sharing one n_blk
     int st, sl;
-    if (per_col >= 1 && m_tiles >= 2 * per_col && plan_smem(block_n, true, slabs, p.num_k_blocks, &st, &sl)) {
+    if (per_col >= 1 && t.m >= 2 * per_col && plan_smem(block_n, true, slabs, p.num_k_blocks, &st, &sl)) {
       plan->bst_stages = plan->stages = st;
       plan->epi_slabs = sl;
-      plan->grid = per_col * n_tiles;   // gridDim.x a multiple of n_tiles: each CTA keeps one n_blk
+      plan->grid = per_col * t.n;   // gridDim.x a multiple of n_tiles: each CTA keeps one n_blk
     }
   }
   return true;
@@ -640,28 +657,14 @@ bool plan_gemm(const GemmProblem& p, int block_n, int num_sms, GemmPlan* plan) {
 
 cudaError_t launch_gemm(const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const CUtensorMap& out, const CUtensorMap& res,
                         const GemmProblem& p, const GemmEpilogue& e, int block_n, const GemmPlan& plan, cudaStream_t stream) {
-  if (plan.bst_stages > 0) {
-    if (block_n == 256) return launch_t<256, true, false>(a0, a1, b, out, res, p, e, plan, stream);
-    if (block_n == 160) return launch_t<160, true, false>(a0, a1, b, out, res, p, e, plan, stream);
-    return launch_t<128, true, false>(a0, a1, b, out, res, p, e, plan, stream);
-  }
-  if (block_n == 256) return launch_t<256, false, false>(a0, a1, b, out, res, p, e, plan, stream);
-  if (block_n == 160) return launch_t<160, false, false>(a0, a1, b, out, res, p, e, plan, stream);
-  return launch_t<128, false, false>(a0, a1, b, out, res, p, e, plan, stream);
+  return launch_any<false>(a0, a1, b, out, res, p, e, block_n, plan, stream);
 }
 
 cudaError_t launch_gemm_fp8(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& out, const CUtensorMap& res, const GemmProblem& p,
                             const GemmEpilogue& e, int block_n, const GemmPlan& plan, cudaStream_t stream) {
   // the 256-wide instantiations have no second accumulator set: they would ignore per-(row, k-block) A scales
   if (e.a_scale_ld != 0 && block_n == 256) return cudaErrorInvalidValue;
-  if (plan.bst_stages > 0) {
-    if (block_n == 256) return launch_t<256, true, true>(a, a, b, out, res, p, e, plan, stream);
-    if (block_n == 160) return launch_t<160, true, true>(a, a, b, out, res, p, e, plan, stream);
-    return launch_t<128, true, true>(a, a, b, out, res, p, e, plan, stream);
-  }
-  if (block_n == 256) return launch_t<256, false, true>(a, a, b, out, res, p, e, plan, stream);
-  if (block_n == 160) return launch_t<160, false, true>(a, a, b, out, res, p, e, plan, stream);
-  return launch_t<128, false, true>(a, a, b, out, res, p, e, plan, stream);
+  return launch_any<true>(a, a, b, out, res, p, e, block_n, plan, stream);
 }
 
 }  // namespace hv

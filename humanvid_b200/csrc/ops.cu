@@ -108,12 +108,13 @@ static int pick_block_n(int64_t N, int64_t m_tiles, bool geglu, int sms) {
   return best;
 }
 
-// Problem block and tile width of the linear out[M, N] = A[M, K] W[N, K]^T: what op_gemm launches and plan_linear reports.
-static GemmProblem linear_problem(int64_t M, int64_t N, int64_t K, bool geglu, int sms, int* block_n) {
+// Problem block and tile width of the linear out[M, N] = A[M, K] W[N, K]^T over k-blocks of kb elements (64 fp16, 128 e4m3): what
+// op_gemm and op_gemm_fp8 launch and plan_linear reports.
+static GemmProblem linear_problem(int64_t M, int64_t N, int64_t K, int kb, bool geglu, int sms, int* block_n) {
   GemmProblem p;
   p.M = static_cast<int>(M);
   p.N = static_cast<int>(N);
-  p.num_k_blocks = static_cast<int>((K + 63) / 64);
+  p.num_k_blocks = static_cast<int>((K + kb - 1) / kb);
   p.a_mode = A_LINEAR;
   *block_n = pick_block_n(N, (M + 127) / 128, geglu, sms);
   return p;
@@ -127,7 +128,7 @@ int plan_linear(int64_t M, int64_t N, int64_t K, bool geglu, int* block_n, int* 
   const int sms = device_sms();
   if (!sms) return HV_ERR_CUDA;
   int bn;
-  const GemmProblem p = linear_problem(M, N, K, geglu, sms, &bn);
+  const GemmProblem p = linear_problem(M, N, K, 64, geglu, sms, &bn);
   GemmPlan plan;
   if (!plan_gemm(p, bn, sms, &plan)) {
     set_error("hv_dbg_gemm_plan: no plan for M=%lld N=%lld K=%lld", (long long)M, (long long)N, (long long)K);
@@ -139,15 +140,16 @@ int plan_linear(int64_t M, int64_t N, int64_t K, bool geglu, int* block_n, int* 
   return HV_OK;
 }
 
-// The launch of a problem the caller has checked and mapped; HV_ERR_INVALID when no plan fits it.
-static int run_gemm(const char* op, const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const CUtensorMap& out,
+// The launch of a problem the caller has checked and mapped (fp8: e4m3 operands, A in a0); HV_ERR_INVALID when no plan fits it.
+// An e4m3 output (e.out8) leaves through register stores only.
+static int run_gemm(const char* op, bool fp8, const CUtensorMap& a0, const CUtensorMap& a1, const CUtensorMap& b, const CUtensorMap& out,
                     const CUtensorMap& res, const GemmProblem& p, const GemmEpilogue& e, int bn, int sms, cudaStream_t stream) {
   GemmPlan plan;
-  if (!plan_gemm(p, bn, sms, &plan)) {
+  if (!plan_gemm(p, bn, sms, &plan) || (e.out8 && plan.epi_slabs)) {
     set_error("%s: no launch plan for M=%d N=%d with %d-column tiles", op, p.M, p.N, bn);
     return HV_ERR_INVALID;
   }
-  return cuda_status(launch_gemm(a0, a1, b, out, res, p, e, bn, plan, stream), op);
+  return cuda_status(fp8 ? launch_gemm_fp8(a0, b, out, res, p, e, bn, plan, stream) : launch_gemm(a0, a1, b, out, res, p, e, bn, plan, stream), op);
 }
 
 int op_gemm(const __half* A, int64_t lda, const __half* A2, int64_t lda2, int64_t K1, const __half* W, __half* out, int64_t ldc,
@@ -173,7 +175,7 @@ int op_gemm(const __half* A, int64_t lda, const __half* A2, int64_t lda2, int64_
   CUtensorMap ma0, ma1, mb;
   const int64_t Ka = split ? K1 : K;
   int bn;
-  GemmProblem p = linear_problem(M, N, K, geglu, sms, &bn);
+  GemmProblem p = linear_problem(M, N, K, 64, geglu, sms, &bn);
   p.k_split = split ? static_cast<int>(K1 / 64) : 0;
   if (!make_map_2d(&ma0, A, M, Ka, lda, 128)) { set_error("hv_op_gemm A map: %s", tma_last_error()); return HV_ERR_TMA; }
   ma1 = ma0;
@@ -183,7 +185,7 @@ int op_gemm(const __half* A, int64_t lda, const __half* A2, int64_t lda2, int64_
   fill_epilogue(e, ep, out, ldc, N);
   CUtensorMap mo, mr;
   if (int rc = make_epilogue_maps("hv_op_gemm", p, e, &mo, &mr)) return rc;
-  return run_gemm("hv_op_gemm", ma0, ma1, mb, mo, mr, p, e, bn, sms, stream);
+  return run_gemm("hv_op_gemm", false, ma0, ma1, mb, mo, mr, p, e, bn, sms, stream);
 }
 
 // e4m3 linear: the checks, then the kernel of op_gemm with KB = 128.  Tile width: GEGLU takes 256 (unpromoted, DESIGN §9); per-128 A
@@ -224,12 +226,9 @@ int op_gemm_fp8(const uint8_t* A, int64_t lda, const float* a_scale, int64_t a_s
   }
   const int sms = device_sms();
   if (!sms) return HV_ERR_CUDA;
-  GemmProblem p;
-  p.M = static_cast<int>(M);
-  p.N = static_cast<int>(N);
-  p.num_k_blocks = static_cast<int>(kblocks);
-  p.a_mode = A_LINEAR;
-  const int bn = a_scale_ld ? ((N + 159) / 160 * 160 <= (N + 127) / 128 * 128 ? 160 : 128) : pick_block_n(N, (M + 127) / 128, geglu, sms);
+  int bn;
+  const GemmProblem p = linear_problem(M, N, K, 128, geglu, sms, &bn);
+  if (a_scale_ld) bn = (N + 159) / 160 * 160 <= (N + 127) / 128 * 128 ? 160 : 128;   // replaces pick_block_n's width (see above)
   CUtensorMap ma, mb;
   if (!make_map_2d_e4m3(&ma, A, M, K, lda, 128)) { set_error("%s A map: %s", op, tma_last_error()); return HV_ERR_TMA; }
   if (!make_map_2d_e4m3(&mb, W, N, K, K, bn)) { set_error("%s W map: %s", op, tma_last_error()); return HV_ERR_TMA; }
@@ -250,12 +249,7 @@ int op_gemm_fp8(const uint8_t* A, int64_t lda, const float* a_scale, int64_t a_s
     fill_epilogue(e, ep, static_cast<__half*>(out), ldc, N);
     if (int rc = make_epilogue_maps(op, p, e, &mo, &mr)) return rc;
   }
-  GemmPlan plan;
-  if (!plan_gemm(p, bn, sms, &plan) || (out_scale && plan.epi_slabs)) {
-    set_error("%s: no launch plan for M=%d N=%d with %d-column tiles", op, p.M, p.N, bn);
-    return HV_ERR_INVALID;
-  }
-  return cuda_status(launch_gemm_fp8(ma, mb, mo, mr, p, e, bn, plan, stream), op);
+  return run_gemm(op, true, ma, ma, mb, mo, mr, p, e, bn, sms, stream);
 }
 
 int op_gemm_batched_b(const __half* A, int64_t lda, const __half* X, int64_t ldx, __half* out, int64_t ldc, int64_t M, int64_t batch,
@@ -285,7 +279,7 @@ int op_gemm_batched_b(const __half* A, int64_t lda, const __half* X, int64_t ldx
   e.ldc = static_cast<int>(ldc);
   e.n_valid = static_cast<int>(rows);
   e.rowbias = rowbias;
-  return run_gemm("hv_op_gemm_batched_b", ma, ma, mb, mb, mb, p, e, bn, sms, stream);
+  return run_gemm("hv_op_gemm_batched_b", false, ma, ma, mb, mb, mb, p, e, bn, sms, stream);
 }
 
 // Tiling of an implicit-GEMM convolution over the NF x H x W grid of the pixels it computes: one M tile is a box of frames x rows x columns.
@@ -332,7 +326,7 @@ int op_conv3x3(const __half* X, const __half* Wp, __half* out, int64_t ldc, int6
   fill_epilogue(e, ep, out, ldc, Cout);
   CUtensorMap mo, mr;
   if (int rc = make_epilogue_maps("hv_op_conv3x3", p, e, &mo, &mr)) return rc;
-  return run_gemm("hv_op_conv3x3", ma, ma, mb, mo, mr, p, e, bn, sms, stream);
+  return run_gemm("hv_op_conv3x3", false, ma, ma, mb, mo, mr, p, e, bn, sms, stream);
 }
 
 // Nearest-2x upsample + 3x3 conv (Upsample3D, resnet.py:68-71 + :49) as four 2x2 convolutions of the SOURCE tensor, one per output
@@ -362,7 +356,7 @@ int op_upconv2x2(const __half* X, const __half* Wp, __half* out, int64_t ldc, in
   if (!make_map_2d(&mb, Wp, 4 * Cout, 4 * Cin, 4 * Cin, bn)) { set_error("hv_op_upconv2x2 W map: %s", tma_last_error()); return HV_ERR_TMA; }
   GemmEpilogue e;
   fill_epilogue(e, ep, out, ldc, Cout);
-  return run_gemm("hv_op_upconv2x2", ma, ma, mb, mb, mb, p, e, bn, sms, stream);
+  return run_gemm("hv_op_upconv2x2", false, ma, ma, mb, mb, mb, p, e, bn, sms, stream);
 }
 
 }  // namespace hv
