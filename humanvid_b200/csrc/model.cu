@@ -197,15 +197,26 @@ struct hv_model {
   // device-resident timestep (CUDA-graph replay of a denoising loop): t = ts_table[*ts_index] when set
   const long long* ts_table = nullptr;
   const int* ts_index = nullptr;
-  // debug taps (error ladder): the activation leaving block i of the forward is copied to tap_dst[i] (channels-last fp16)
+  // debug taps (per-block parity, error ladder): the activation leaving block `name` of a forward is copied to tap_dst[i] (channels-last
+  // fp16, all C channels including any padding), i = the entry of `name` in the plan that the planning pass leaves in tap_list.  A VAE
+  // handle plans a decode and then an encode (the decoder's taps, then the encoder's), so a forward finds its entries by name.  With no
+  // taps set a forward issues nothing more.
   struct TapInfo { std::string name; int NF, H, W, C; };
   std::vector<TapInfo> tap_list;
   std::vector<void*> tap_dst;
-  void tap(const std::string& name, const Tens& t) {   // records the plan entry in the planning pass too (hv_debug_tap_count)
-    const size_t i = tap_list.size();
-    tap_list.push_back({name, t.NF, t.H, t.W, t.C});
-    if (i < tap_dst.size() && tap_dst[i] != nullptr)
-      launch(1, {}, [&] { ck(cudaMemcpyAsync(tap_dst[i], t.p, static_cast<size_t>(t.numel()) * 2, cudaMemcpyDeviceToDevice, st), "tap copy"); });
+  void tap(const std::string& name, const Tens& t) {
+    if (ar.dry) {
+      tap_list.push_back({name, t.NF, t.H, t.W, t.C});
+      return;
+    }
+    for (size_t i = 0; i < tap_dst.size() && i < tap_list.size(); ++i) {
+      const TapInfo& e = tap_list[i];
+      if (e.name != name) continue;
+      if (e.NF != t.NF || e.H != t.H || e.W != t.W || e.C != t.C) fail(HV_ERR_STATE, "tap '%s' does not match its plan entry", name.c_str());
+      if (tap_dst[i] != nullptr)
+        launch(1, {}, [&] { ck(cudaMemcpyAsync(tap_dst[i], t.p, static_cast<size_t>(t.numel()) * 2, cudaMemcpyDeviceToDevice, st), "tap copy"); });
+      return;
+    }
   }
   // optional per-category device timing (bench.py's roofline): events bracket every categorised operator launch
   enum Cat { CAT_NONE = -1, CAT_GEMM = 0, CAT_CONV = 1, CAT_ATTN = 2, CAT_TATTN = 3, CAT_NORM = 4, CAT_MISC = 5, CAT_N = 6 };
@@ -1019,8 +1030,8 @@ struct hv_model {
     ar.dry = dry;
     ar.off = 0;
     ar.peak = 0;
-    tap_list.clear();
     if (dry) {
+      tap_list.clear();
       ar.base = nullptr;
       ar.cap = 0;
     } else {   // a planning pass keeps the launch count and the profile of the last forward
@@ -1108,9 +1119,11 @@ struct hv_model {
         ckop(op_conv3x3_direct(x0.p, pg_in.w, pg_in.bias, h.p, NF, H, W, pg_in.cin, pg_in.cout, 1, HV_ACT_SILU, nullptr, h.C, st), "pose conv_in");
       });
     }
+    tap("conv_in", h);
     for (size_t i = 0; i < pg_convs.size(); ++i) {
       const bool last = i + 1 == pg_convs.size();
       const Conv3& c = pg_convs[i];
+      const std::string name = last ? "conv_out" : "blocks." + std::to_string(i);
       if (pg_small[i]) {
         // the next layer either is a small-channel layer too (dense channels) or the first implicit-GEMM layer (its 64-multiple k-blocks)
         const int ld = pg_small[i + 1] ? c.cout : pg_convs[i + 1].cin_pad;
@@ -1121,11 +1134,13 @@ struct hv_model {
         launch(1, {CAT_CONV, pg_strides[i] == 1 ? "smallconv" : "smallconv_s2", 2.0 * out.rows() * c.cout * 9.0 * c.cin, out.rows(), c.cout, 9LL * c.cin},
                [&] { ckop(op_conv3x3_small(h.p, c.w.p, c.bias, out.p, ld, NF, h.H, h.W, c.cin, c.cout, pg_strides[i], HV_ACT_SILU, st), "pose small conv"); });
         h = out;
+        tap(name, h);
         continue;
       }
       h = op_conv3(h, c, pg_strides[i], nullptr, nullptr, last ? HV_ACT_NONE : HV_ACT_SILU);
       // the next conv expects cin_pad channels: cout_pad of this conv equals it by construction (both round to 64)
       if (!last && h.C != pg_convs[i + 1].cin_pad) fail(HV_ERR_INVALID, "pose guider channel padding mismatch at conv %zu", i);
+      tap(name, h);
     }
     launch(1, {}, [&] { ckop(op_nhwc_to_ncfhw(h.p, h.C, outp, B, cfg.pg_out_channels, F, h.H, h.W, st), "pose output layout"); });
   }
@@ -1143,13 +1158,18 @@ struct hv_model {
         ckop(op_pixel_unshuffle(plucker, u.p, B, cin0, F, H, W, r, st), "pixel unshuffle");
     });
     Tens x = op_conv3(u, cam_in);
+    tap("encoder_conv_in", x);
     for (int j = 0; j < cfg.cam_nums_rb; ++j) {
+      const std::string sj = ".0." + std::to_string(j);
       // ResnetBlock (pose_adaptor.py:102-135, sk=True, ksize=1): x = block2(relu(block1(x))) + x
       Tens h1 = op_conv3(x, cam_res[j].block1, 1, nullptr, nullptr, HV_ACT_RELU);
       x = op_linear(h1, cam_res[j].block2, &x);
+      tap("encoder_down_conv_blocks" + sj, x);
       x = tblock_fwd(cam_att[j], x, B, F);   // over the frame axis
+      tap("encoder_down_attention_blocks" + sj, x);
     }
     Tens z = op_linear(x, cam_zero);
+    tap("zero_conv_layers.0", z);
     launch(1, {}, [&] { ckop(op_nhwc_to_ncfhw(z.p, z.C, outp, NF, C, 1, z.H, z.W, st), "camera output layout"); });
   }
 
@@ -1157,12 +1177,32 @@ struct hv_model {
   // UNetMidBlock2D: resnet, attention (diffusers Attention: GroupNorm, self-attention + residual), resnet
   Tens vae_mid_fwd(const VaeHalf& v, Tens h) {
     h = resnet_fwd(v.mid.res[0], h, nullptr, nullptr, h.NF, 1);
+    tap(v.mid.name + ".resnets.0", h);
     Tens a = alloc_act(h.NF, h.H, h.W, h.C);
     {
       Scope s(ar);
       self_attn_fwd(v.attn, op_gn(h, nullptr, v.attn_gn, false), h, a, [] { return BankKV{}; });
     }
-    return resnet_fwd(v.mid.res[1], a, nullptr, nullptr, a.NF, 1);
+    tap(v.mid.name + ".attentions.0", a);
+    h = resnet_fwd(v.mid.res[1], a, nullptr, nullptr, a.NF, 1);
+    tap(v.mid.name + ".resnets.1", h);
+    return h;
+  }
+  // the resnets and the sampler of one encoder / decoder stage
+  Tens vae_stage_fwd(const Stage& s, Tens h, int N, bool down) {
+    for (size_t j = 0; j < s.res.size(); ++j) {
+      h = resnet_fwd(s.res[j], h, nullptr, nullptr, N, 1);
+      tap(s.name + ".resnets." + std::to_string(j), h);
+    }
+    if (!s.has_sampler) return h;
+    if (down) {
+      h = op_conv3(h, s.sampler, 2, nullptr, nullptr, HV_ACT_NONE, nullptr, 1, true);   // Downsample2D: pad (0, 1, 0, 1), stride 2
+      tap(s.name + ".downsamplers.0", h);
+    } else {
+      h = op_upconv(h, s.sampler);
+      tap(s.name + ".upsamplers.0", h);
+    }
+    return h;
   }
   // Every operator works per frame (per-frame GroupNorm statistics, per-frame attention), so frame i of a call does not depend on the
   // other frames of the call.
@@ -1170,28 +1210,30 @@ struct hv_model {
     if (N <= 0 || H <= 0 || W <= 0 || (H % 8) || (W % 8)) fail(HV_ERR_INVALID, "AutoencoderKL.encode: N = %d images of %dx%d: N must be > 0 and H, W positive multiples of 8", N, H, W);
     Tens x0 = padded_input(x, N, cfg.in_channels, 1, H, W, enc.conv_in.cin_pad);
     Tens h = op_conv3(x0, enc.conv_in);
-    for (const Stage& s : enc.blocks) {
-      for (const ResnetW& r : s.res) h = resnet_fwd(r, h, nullptr, nullptr, N, 1);
-      if (s.has_sampler) h = op_conv3(h, s.sampler, 2, nullptr, nullptr, HV_ACT_NONE, nullptr, 1, true);   // Downsample2D: pad (0, 1, 0, 1), stride 2
-    }
+    tap("encoder.conv_in", h);
+    for (const Stage& s : enc.blocks) h = vae_stage_fwd(s, h, N, true);
     h = vae_mid_fwd(enc, h);
     Tens hn = op_gn(h, nullptr, enc.norm_out, true);
+    tap("encoder.conv_norm_out", hn);
     Tens y = op_conv3(hn, enc.conv_out);
+    tap("encoder.conv_out", y);
     Tens m = op_linear(y, quant);   // quant_conv (1x1)
+    tap("quant_conv", m);
     launch(1, {}, [&] { ckop(op_nhwc_to_ncfhw(m.p, m.C, moments, N, m.C, 1, m.H, m.W, st), "moments layout"); });
   }
   void vae_decode(const __half* z, __half* outp, int N, int H, int W) {
     if (N <= 0 || H <= 0 || W <= 0) fail(HV_ERR_INVALID, "AutoencoderKL.decode: N = %d latents of %dx%d must all be positive", N, H, W);
     Tens z0 = padded_input(z, N, cfg.vae_latent_channels, 1, H, W, static_cast<int>(post_quant.w.cols));
     Tens p = op_linear(z0, post_quant);   // post_quant_conv (1x1); its padded channels stay zero for conv_in
+    tap("post_quant_conv", p);
     Tens h = op_conv3(p, dec.conv_in);
+    tap("decoder.conv_in", h);
     h = vae_mid_fwd(dec, h);
-    for (const Stage& s : dec.blocks) {
-      for (const ResnetW& r : s.res) h = resnet_fwd(r, h, nullptr, nullptr, N, 1);
-      if (s.has_sampler) h = op_upconv(h, s.sampler);
-    }
+    for (const Stage& s : dec.blocks) h = vae_stage_fwd(s, h, N, false);
     Tens hn = op_gn(h, nullptr, dec.norm_out, true);
+    tap("decoder.conv_norm_out", hn);
     Tens y = op_conv3(hn, dec.conv_out);
+    tap("decoder.conv_out", y);
     launch(1, {}, [&] { ckop(op_nhwc_to_ncfhw(y.p, y.C, outp, N, cfg.out_channels, 1, y.H, y.W, st), "image output layout"); });
   }
 
@@ -1225,11 +1267,13 @@ struct hv_model {
     Tens x = alloc_act(B, 1, L, C);
     launch(1, {CAT_NORM, "clip_embed_ln", 0, x.rows(), C, 0},
            [&] { ckop(op_clip_embed_ln(pe.p, clip_cls, clip_pos, clip_pre.g, clip_pre.b, x.p, x.rows(), L, C, clip_pre.eps, st), "embeddings + pre_layrnorm"); });
+    tap("vision_model.pre_layrnorm", x);
     for (size_t i = 0; i < clip_layers.size(); ++i) {
       const bool last = i + 1 == clip_layers.size();
       __half* dst = last && lhs != nullptr ? lhs : x.p;   // the stream is updated in place; the last layer writes the caller's last_hidden_state
       clip_layer_fwd(clip_layers[i], x, dst);
       x.p = dst;
+      tap("vision_model.encoder.layers." + std::to_string(i), x);
     }
     // pooling: the class token of each image -> post_layernorm -> visual_projection (no bias)
     Tens cls = alloc_act(B, 1, 1, C);
@@ -1238,6 +1282,7 @@ struct hv_model {
          "class tokens");
     });
     Tens pooled = op_ln(cls, clip_post);
+    tap("vision_model.post_layernorm", pooled);
     const int P = static_cast<int>(clip_proj.rows);
     launch(1, {CAT_MISC, "", 2.0 * B * P * C},
            [&] { ckop(hv::op_small_linear(pooled.p, clip_proj.p, nullptr, embeds, B, P, C, HV_ACT_NONE, st), "visual_projection"); });
@@ -1287,7 +1332,7 @@ static size_t measure(hv_model* h, int B, int F, int H, int W, uint32_t flags = 
   } else if (h->cfg.kind == HV_KIND_VAE) {   // (H, W) = latent size: the workspace covers decoding B latents and encoding B images of 8H x 8W
     h->vae_decode(nullptr, nullptr, B, H, W);
     const size_t dec_peak = h->ar.peak;
-    h->begin(nullptr, 0, true, nullptr);
+    h->ar.off = h->ar.peak = 0;   // the encode on an empty arena; its taps follow the decoder's in tap_list
     h->vae_encode(nullptr, nullptr, B, 8 * H, 8 * W);
     return std::max(dec_peak, h->ar.peak) + 4096;
   } else if (h->cfg.kind == HV_KIND_CLIP_VISION) {   // (B, 1, S, S): B images of S x S pixels

@@ -436,6 +436,32 @@ class _NativeNet(nn.Module):
             return 0
         return int(N.lib().hv_last_launch_count(self._handle))
 
+    # ---- debug taps (per-block parity tests, scripts/error_ladder.py) ------------------------------------------------------
+    def debug_tap_plan(self, B, F, h, w):
+        """[(reference module path, (NF, H, W, C))] of the activations the native forward can copy out, in execution order, at the shape
+        ``hv_workspace_bytes`` takes: (B, F, h, w) latent for the UNets (F = 1 for the 2-D one), (n, 1, h, w) latent for the VAE (the
+        decoder's taps at h x w, then the encoder's at 8h x 8w), (B, 1, S, S) for CLIP, (B, F, H, W) image for the PoseGuider and the
+        camera encoder.  C includes the zero channels of a padded layout."""
+        hd = self._sync_native()
+        lib = N.lib()
+        n = lib.hv_debug_tap_count(hd, N.i32(B), N.i32(F), N.i32(h), N.i32(w))
+        if n < 0:
+            N.check(n, hd)
+        plan = []
+        for i in range(n):
+            name = C.create_string_buffer(128)
+            dims = (C.c_int64 * 4)()
+            N.check(lib.hv_debug_tap_info(hd, N.i32(i), name, N.i32(128), dims), hd)
+            plan.append((name.value.decode(), tuple(int(d) for d in dims)))
+        return plan
+
+    def debug_set_taps(self, tensors):
+        """tensors[i] (or None) receives tap i of ``debug_tap_plan`` as channels-last fp16 (NF, H, W, C) on the next forwards; [] disables."""
+        hd = self._sync_native()
+        self._tap_refs = list(tensors)
+        arr = (C.c_void_p * max(len(tensors), 1))(*[None if t is None else t.data_ptr() for t in tensors])
+        N.check(N.lib().hv_debug_set_taps(hd, arr if tensors else None, N.i32(len(tensors))), hd)
+
 
 class HvConfig(C.Structure):
     _fields_ = [
@@ -616,29 +642,6 @@ class UNet3DConditionModel(_NativeNet):
             self.__dict__["_fp8"] = bool(on)
             self._epoch = getattr(self, "_epoch", 0) + 1
 
-    # ---- debug taps (per-layer error ladder; scripts/error_ladder.py) ---------------------------------------------------
-    def debug_tap_plan(self, B, F, h, w):
-        """[(reference module path, (NF, H, W, C))] of the activations the native forward can copy out, in execution order."""
-        hd = self._sync_native()
-        lib = N.lib()
-        n = lib.hv_debug_tap_count(hd, N.i32(B), N.i32(F), N.i32(h), N.i32(w))
-        if n < 0:
-            N.check(n, hd)
-        plan = []
-        for i in range(n):
-            name = C.create_string_buffer(128)
-            dims = (C.c_int64 * 4)()
-            N.check(lib.hv_debug_tap_info(hd, N.i32(i), name, N.i32(128), dims), hd)
-            plan.append((name.value.decode(), tuple(int(d) for d in dims)))
-        return plan
-
-    def debug_set_taps(self, tensors):
-        """tensors[i] (or None) receives tap i as channels-last fp16 (NF, H, W, C) on the next forwards; [] disables."""
-        hd = self._sync_native()
-        self._tap_refs = list(tensors)
-        arr = (C.c_void_p * max(len(tensors), 1))(*[None if t is None else t.data_ptr() for t in tensors])
-        N.check(N.lib().hv_debug_set_taps(hd, arr if tensors else None, N.i32(len(tensors))), hd)
-
     def workspace_bytes(self, B, F, h, w) -> int:
         return self._workspace_bytes(B, F, h, w)
 
@@ -775,10 +778,6 @@ class UNet2DConditionModel(_NativeNet):
 
     def _hv_config(self):
         return _sd15_hv_config(self.config, N.HV_KIND_UNET2D_REF)
-
-    # debug taps: the denoising UNet's, at one frame (debug_tap_plan(B, 1, h, w))
-    debug_tap_plan = UNet3DConditionModel.debug_tap_plan
-    debug_set_taps = UNet3DConditionModel.debug_set_taps
 
     @torch.no_grad()
     def forward(self, sample: torch.Tensor, timestep: Union[torch.Tensor, float, int], encoder_hidden_states: torch.Tensor,

@@ -167,10 +167,19 @@ int hv_vae_encode(hv_handle h, const void* x, void* moments, int32_t N, int32_t 
 int hv_clip_vision_forward(hv_handle h, const void* pixel_values, void* image_embeds, void* last_hidden_state, int32_t B, void* workspace,
                            size_t ws_bytes, hv_stream_t stream);
 
-/* Debug taps (per-layer error ladder, scripts/error_ladder.py): the activation leaving the i-th block of the UNet forward (conv_in, every
- * resnet / transformer / motion module / down- / up-sampler, in execution order) is copied to dst[i] as channels-last fp16
- * (NF, H, W, C).  hv_debug_tap_count plans the forward at this shape and returns the number of taps; hv_debug_tap_info
- * names tap i (the reference's module path) and gives dims4 = {NF, H, W, C}; hv_debug_set_taps(h, NULL, 0) disables. */
+/* Debug taps (per-block parity tests, scripts/error_ladder.py): the activation leaving each block of a forward is copied to dst[i] as
+ * channels-last fp16 (NF, H, W, C), C including the zero channels a padded layout carries.  The blocks, in execution order:
+ *   UNets          conv_in, every resnet / transformer / motion module / down- / up-sampler
+ *   AutoencoderKL  the decoder's (post_quant_conv, decoder.conv_in, the mid block's resnets and attention, every up-block resnet and
+ *                  upsampler, decoder.conv_norm_out (GroupNorm + SiLU), decoder.conv_out), then the encoder's (encoder.conv_in, ...,
+ *                  encoder.conv_out, quant_conv); a decode fills only the decoder's entries and an encode only the encoder's
+ *   CLIP vision    vision_model.pre_layrnorm (B, 1, L, C), every vision_model.encoder.layers.i, vision_model.post_layernorm (B, 1, 1, C)
+ *   PoseGuider     conv_in, blocks.0 .. blocks.5, conv_out (before the output layout pass)
+ *   camera encoder encoder_conv_in, then per resnet / attention pair encoder_down_conv_blocks.0.j, encoder_down_attention_blocks.0.j,
+ *                  zero_conv_layers.0 (hv_camera_encoder_forward and _forward_rays alike)
+ * hv_debug_tap_count plans the forward at the shape hv_workspace_bytes takes and returns the number of taps; hv_debug_tap_info names
+ * tap i (the reference's module path) and gives dims4 = {NF, H, W, C}; hv_debug_set_taps(h, NULL, 0) disables.  With no taps set a
+ * forward launches nothing more. */
 int hv_debug_tap_count(hv_handle h, int32_t B, int32_t F, int32_t height, int32_t width);
 int hv_debug_tap_info(hv_handle h, int32_t i, char* name, int32_t name_cap, int64_t* dims4);
 int hv_debug_set_taps(hv_handle h, void* const* dst, int32_t n);

@@ -1,5 +1,6 @@
-"""Per-slice, per-row and per-element checks of one UNet block's output against a high-precision reference, shared by
-tests/test_block_parity_gpu.py (native taps of the whole UNet) and tests/test_block_parity_cpu.py (the checks' self-test).
+"""Per-slice, per-row and per-element checks of one native block's output against a high-precision reference, shared by
+tests/test_block_parity_gpu.py (native taps of the whole UNet), tests/test_net_block_parity_gpu.py (the VAE, CLIP, PoseGuider and camera
+encoder) and the CPU self-tests tests/test_block_parity_cpu.py and tests/test_net_block_parity_cpu.py.
 
 A tap is (NF, H, W, C): NF = batch items x frames.  A slice s is one (item, frame), all H W C elements; a row r one token of it.  For a
 block whose output N and the fp16 eager result E are compared with the fp64 result R of the same block on the same input:
@@ -18,6 +19,9 @@ For a block whose feed-forward runs on e4m3 (FP8 mode) R is replaced by the e4m3
 budget of tests/test_fp8_model_gpu.py, rel_s(N8, Emu) <= 0.6 rel_s(Emu, R) + 2^-10; the row and element bounds add ``extra`` (see
 tests/fp8_emulation.ff_flip_bound).  That term is the worst case of every GEGLU value of a token flipping at once, far above what flips
 do, so for these blocks the slice budget is the tight check and the row and element bounds catch only gross faults.
+
+A tap whose layout carries padding channels (the 64-channel input of an implicit-GEMM conv, a conv output rounded up to 8 channels) is
+compared on its true channels, and every padding channel must be exactly zero (check_pad).
 """
 from dataclasses import dataclass, field
 
@@ -82,12 +86,13 @@ class BlockReport:
     e_row: Worst = field(default_factory=Worst)     # the fp16 eager result against the row and element bounds
     e_elem: Worst = field(default_factory=Worst)
     nonfinite: list = field(default_factory=list)
+    pad: list = field(default_factory=list)         # taps with a padding channel that is not exactly zero
 
     def worst(self):
         return max(self.slice.ratio, self.row.ratio, self.elem.ratio)
 
     def failures(self, with_eager=True):
-        out = [f"non-finite output in {n}" for n in self.nonfinite]
+        out = [f"non-finite output in {n}" for n in self.nonfinite] + [f"non-zero padding channel in {p}" for p in self.pad]
         checks = [("slice", self.slice), ("row", self.row), ("element", self.elem)]
         if with_eager:
             checks += [("fp16-eager row", self.e_row), ("fp16-eager element", self.e_elem)]
@@ -125,7 +130,32 @@ def check_fp8_block(rep: BlockReport, label: str, N8, Emu, R, extra):
     rep.elem.take(elem_ratio(N8, Emu, extra), label)
 
 
-def block_kind(name: str) -> str:
-    """The kind of a tap: conv_in, resnets, attentions, motion_modules, downsamplers, upsamplers."""
-    return "conv_in" if name == "conv_in" else name.split(".")[-2]
+def check_pad(rep: BlockReport, label: str, N, c: int):
+    """Add the padding channels c.. of a native tap N (NF, H, W, C) to rep: each must be +0 or -0.  The next implicit-GEMM conv reads them
+    through zero weight columns, and 0 * NaN or 0 * Inf would reach its real outputs."""
+    bad = (N[..., c:] != 0).nonzero()                # NaN != 0 too
+    if len(bad):
+        n, h, w, ch = (int(i) for i in bad[0])
+        rep.pad.append(f"{label} (slice, h, w, channel) = {(n, h, w, c + ch)}, {len(bad)} elements")
 
+
+# tap names of the VAE, CLIP, PoseGuider and camera encoder that do not end in "<kind>.<index>": whole names, last components, prefixes
+_NAMED = {"post_quant_conv": "conv1x1", "quant_conv": "conv1x1", "zero_conv_layers.0": "conv1x1", "vision_model.pre_layrnorm": "clip_embed",
+          "vision_model.post_layernorm": "clip_pool"}
+_LAST = {"conv_in": "conv_in", "encoder_conv_in": "conv_in", "conv_out": "conv_out", "conv_norm_out": "norm_out"}
+_PREFIX = (("vision_model.encoder.layers.", "clip_layer"), ("blocks.", "pg_conv"), ("encoder_down_conv_blocks.", "cam_res"),
+           ("encoder_down_attention_blocks.", "cam_attn"))
+
+
+def block_kind(name: str) -> str:
+    """The kind of a tap: conv_in, resnets, attentions, motion_modules, downsamplers, upsamplers (UNets, VAE), norm_out (GroupNorm + SiLU),
+    conv_out, conv1x1, clip_embed, clip_layer, clip_pool, pg_conv (PoseGuider blocks), cam_res, cam_attn (camera encoder)."""
+    if name in _NAMED:
+        return _NAMED[name]
+    last = name.rsplit(".", 1)[-1]
+    if last in _LAST:
+        return _LAST[last]
+    for prefix, kind in _PREFIX:
+        if name.startswith(prefix):
+            return kind
+    return name.split(".")[-2]
